@@ -1,15 +1,15 @@
 #!/usr/bin/env python
-"""Benchmark of the W4A16 linear path (BASELINE.json metric): Llama-3-8B W4A16 g128, 1 x B200.
+"""Benchmark of the W4A16 linear path (BASELINE.json metric): Llama-3-8B W4A16 g128, 1 x H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference|reference-gpu]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference|reference-gpu] [--dump-outputs DIR]
 
 A "step" is ONE pass of the hot path over one batch of synthetic input:
   decode  (headline, BASELINE configs[1]): the 160 W4A16 GEMVs of one token, 32 layers x
           {qkv 4096->6144, o 4096->4096, gate/up 4096->14336, down 14336->4096}, M = 1, all 32
-          layers' weights distinct (3.7 GB >> the 126 MB L2, so every weight byte is an HBM read;
+          layers' weights distinct (3.7 GB >> the 50 MB L2, so every weight byte is an HBM read;
           that is the "inputs larger than L2" timing rule), executed in model order.
   prefill (BASELINE configs[2], reported in the same line under "prefill"): the same 160 layers
-          with M = 2048 tokens through the tcgen05 tensor-core kernel.
+          with M = 2048 tokens through the wgmma tensor-core kernel.
 `value`  = tokens/s of the linear path with inputs resident in HBM: the 160 launches of a step are a
            CUDA graph of C-ABI launches (include/b200awq.h), K steps timed with CUDA events.
 `e2e`    = the same metric through the reference-facing plugin (`awq_inference_engine.
@@ -19,6 +19,10 @@ A "step" is ONE pass of the hot path over one batch of synthetic input:
 Synthetic data: random int16 packed weights (every bit pattern is a legal packing), scales
 0.004..0.016, integer zero points, N(0,1) activations (SURVEY.md §8d).  Multi-GPU: the model fits
 one GPU, so N ranks are N independent replicas (no data-path collective; "scaling": "weak").
+Every timed window runs exactly K steps after W warm-up steps.  --dump-outputs DIR writes what the last timed step
+of each timed path returned to its caller as DIR/<name>.npy (float32; the 2048-token prefill outputs as a fixed,
+seeded sample of 256 token rows), for comparing two builds output for output: the inputs are seeded and identical
+from run to run.
 """
 import argparse
 import ctypes
@@ -35,7 +39,7 @@ if ROOT not in sys.path:
 
 LLAMA3_8B = dict(name="Llama-3-8B", hidden=4096, inter=14336, q_heads=32, kv_heads=8, head_dim=128, layers=32)
 LLAMA2_70B = dict(name="Llama-2-70B", hidden=8192, inter=28672, q_heads=64, kv_heads=8, head_dim=128, layers=80)
-METRIC = "Llama-3-8B W4A16 g128 decode tok/s (linear path), %dxB200"
+METRIC = "Llama-3-8B W4A16 g128 decode tok/s (linear path), %dxH100"
 UNIT = "tok/s"
 G = 128
 
@@ -62,11 +66,9 @@ def scale_rows(K):
 
 
 def read_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return dict(hbm=d["hbm_gbs"], tc_burst=d["bf16_tflops"], tc_sustained=d["bf16_tflops_sustained"], source="measured")
-    return dict(hbm=6650.0, tc_burst=1590.0, tc_sustained=1400.0, source="fallback")
+    """NVIDIA's data-sheet figures for the H100 SXM (700 W): HBM3 bandwidth and dense fp16 / bf16 tensor-core rate.
+    A card with a lower power limit reaches less; the clocks record of the result line says what the card ran at."""
+    return dict(hbm=3350.0, tc_burst=989.0, tc_sustained=989.0, source="H100 SXM data sheet")
 
 
 # ------------------------------------------------------------------------------------------ clocks
@@ -206,6 +208,27 @@ def timed_steps(torch, dist, device, step_fn, steps, warmup, sync_each=False):
     return max_over_ranks(torch, dist, ms, device), (t0, t1)
 
 
+DUMP_BYTES = 64 << 20
+PREFILL_DUMP_ROWS = 256
+
+
+def dump_outputs(out_dir, arrays):
+    """arrays: name -> tensor.  Written as float32 .npy, at most DUMP_BYTES in all."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    total = sum(t.numel() * 4 for t in arrays.values())
+    if total > DUMP_BYTES:
+        raise RuntimeError("--dump-outputs: %d bytes exceed the %d-byte limit" % (total, DUMP_BYTES))
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
+
+
+def prefill_sample_rows(torch, M):
+    """The fixed, seeded sample of token rows dumped from a prefill output."""
+    g = torch.Generator().manual_seed(2048)
+    return torch.randperm(M, generator=g)[:PREFILL_DUMP_ROWS].sort().values
+
+
 # ------------------------------------------------------------------------------------------ arms
 def run_b200(args):
     import torch
@@ -277,12 +300,13 @@ def run_b200(args):
 
     def eager_e2e(M, steps):
         """The SAME end-to-end step without a CUDA graph: every layer is one eager call of the reference-facing module
-        (the reference's own, unmodified WQLinear.forward when baseline/_ref is staged, else this repo's mirror), as
-        tinychat / awq.entry make them; pinned H2D of the activations and D2H of the result every step."""
+        (this repo's mirror of WQLinear.forward), as tinychat / awq.entry make them; pinned H2D of the activations and
+        D2H of the result every step."""
         mods, kind = reference_wqlinears(torch, model, device, dtype)
         hx = {K: v.cpu().pin_memory() for K, v in make_inputs(M).items()}
         dx = {K: torch.empty_like(v, device=device).view(1, M, K) for K, v in hx.items()}
         hy = torch.empty(1, M, cfg["hidden"], dtype=dtype).pin_memory()
+        eager_out["y"] = hy
 
         def step():
             for K in dx:
@@ -293,7 +317,7 @@ def run_b200(args):
             hy.copy_(y, non_blocking=True)
             torch.cuda.current_stream().synchronize()
             _ = float(hy[0, 0, 0])
-        ms, w = timed_steps(torch, dist, device, step, steps, 5)
+        ms, w = timed_steps(torch, dist, device, step, steps, args.warmup)
         # host cost of one call when the GPU is not the bottleneck: issue the calls of one step and stop the clock before
         # waiting for the device
         torch.cuda.synchronize()
@@ -331,8 +355,8 @@ def run_b200(args):
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g):
                     launch_all()
-                ms, _ = timed_steps(torch, None, device, g.replay, 20, 3)
-                us = ms * 1e3 / 20 / len(layers)
+                ms, _ = timed_steps(torch, None, device, g.replay, args.steps, args.warmup)
+                us = ms * 1e3 / args.steps / len(layers)
                 row["%dx%d" % (N, K)] = {"us": round(us, 3), "frac": round(alg_bytes(M, N, K) / us / 1e3 / peaks["hbm"], 4),
                                          "calls": len(layers)}
             tot_us = sum(v["us"] * v["calls"] for v in row.values())
@@ -341,6 +365,7 @@ def run_b200(args):
             out[str(M)] = row
         return out
 
+    eager_out = {}
     sampler.start()
     # ---------------- decode: device-resident
     g_dec, keep1 = abi_graph(1, "gemv")
@@ -357,9 +382,9 @@ def run_b200(args):
     windows.append(w)
     # ---------------- prefill (secondary object)
     Mp = 2048
-    ksteps_p = max(3, min(args.steps, args.prefill_steps))
+    ksteps_p = args.steps
     g_pre, keep2 = abi_graph(Mp, "gemm")
-    ms_pre, w = timed_steps(torch, dist, device, g_pre.replay, ksteps_p, 3)
+    ms_pre, w = timed_steps(torch, dist, device, g_pre.replay, ksteps_p, args.warmup)
     windows.append(w)
     g_pe2e, hyp, h2dp, d2hp = plugin_graph(Mp, "gemm")
 
@@ -367,11 +392,20 @@ def run_b200(args):
         g_pe2e.replay()
         torch.cuda.current_stream().synchronize()
         _ = float(hyp[0, 0])
-    ms_pe2e, w = timed_steps(torch, dist, device, pe2e_step, ksteps_p, 3)
+    ms_pe2e, w = timed_steps(torch, dist, device, pe2e_step, ksteps_p, args.warmup)
     windows.append(w)
     # ---------------- decode end to end WITHOUT a graph (what an unmodified caller sees)
-    ms_eager, host_us, eager_kind, w = eager_e2e(1, min(args.steps, 100))
+    ms_eager, host_us, eager_kind, w = eager_e2e(1, args.steps)
     windows.append(w)
+    if args.dump_outputs and rank == 0:
+        rows = prefill_sample_rows(torch, Mp).to(device)
+        out = {"decode_y_n%d" % N: y for N, y in keep1[1].items()}
+        out.update({"prefill_y_n%d_rows" % N: y.index_select(0, rows) for N, y in keep2[1].items()})
+        out["decode_e2e_y"] = hy
+        out["prefill_e2e_y_rows"] = hyp.index_select(0, rows.cpu())
+        out["decode_eager_y"] = eager_out["y"].view(1, -1)
+        out["prefill_sample_rows"] = rows
+        dump_outputs(args.dump_outputs, out)
     sweep = batch_sweep() if (world == 1 and args.sweep) else None
     clocks = sampler.stop(windows)
     tp = None
@@ -382,16 +416,13 @@ def run_b200(args):
         del g_dec, g_e2e, g_pre, g_pe2e, keep1, keep2
         model.clear()
         torch.cuda.empty_cache()
-        tp = tp70b_measure(torch, dist, rank, world, device, min(args.steps, 100), args.warmup)
+        tp = tp70b_measure(torch, dist, rank, world, device, args.steps, args.warmup)
 
     if rank != 0:
         return
     step_ms = ms_dec / args.steps
     ach = bytes_step / (step_ms * 1e-3) / 1e9
     traffic = None
-    tf = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tf):
-        traffic = json.load(open(tf)).get("decode_dram_bytes_per_launch")
     pre_ms = ms_pre / ksteps_p
     tfl = flops_step / (pre_ms * 1e-3) / 1e12
     line = {
@@ -410,7 +441,7 @@ def run_b200(args):
                       "api": eager_kind + ".forward x160, eager launches (no CUDA graph), pinned H2D/D2H + host read every step"},
         "gpu_launches": nl * args.steps,
         "roofline": {"bound": "hbm", "achieved": ach, "peak": peaks["hbm"], "unit": "GB/s", "frac": ach / peaks["hbm"],
-                     "traffic": traffic, "kernel": "w4a16_decode_kernel", "peak_source": peaks["source"] + " (burst copy)",
+                     "traffic": traffic, "kernel": "w4a16_decode_kernel", "peak_source": peaks["source"],
                      "bytes_per_launch": bytes_step / nl, "avg_launch_us": step_ms * 1e3 / nl},
         "clocks": clocks,
         "prefill": {"metric": "Llama-3-8B W4A16 g128 prefill tok/s (linear path), seq=2048 (BASELINE configs[2])",
@@ -419,55 +450,35 @@ def run_b200(args):
                             "d2h_bytes_per_step": d2hp},
                     "gpu_launches": nl * ksteps_p,
                     "roofline": {"bound": "tensor", "achieved": tfl, "peak": peaks["tc_sustained"], "unit": "TFLOP/s",
-                                 "frac": tfl / peaks["tc_sustained"], "traffic": None, "kernel": "w4a16_umma_kernel",
-                                 "peak_source": peaks["source"] + " (sustained cuBLAS bf16)", "frac_of_burst": tfl / peaks["tc_burst"]}},
+                                 "frac": tfl / peaks["tc_sustained"], "traffic": None, "kernel": "w4a16_wgmma_kernel",
+                                 "peak_source": peaks["source"], "frac_of_burst": tfl / peaks["tc_burst"]}},
     }
     if sweep is not None:
         line["batch_sweep"] = sweep
     if tp is not None:
         line["tp70b"] = tp
-    ptf = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(ptf):
-        line["prefill"]["roofline"]["traffic"] = json.load(open(ptf)).get("prefill_dram_bytes_per_launch")
     if world == 1 and not args.no_cpu:
         line["cpu_baseline"] = cpu_baseline(args.cpu_seconds)
     if world == 1 and args.ref_gpu:
         try:
-            line["reference_on_b200"] = reference_gpu(torch, model, make_inputs, device, min(args.steps, 200), lib)
+            line["reference_on_gpu"] = reference_gpu(torch, model, make_inputs, device, args.steps, args.warmup, lib)
         except Exception as e:  # noqa: BLE001
-            line["reference_on_b200"] = {"unavailable": repr(e)[:200]}
+            line["reference_on_gpu"] = {"unavailable": repr(e)[:200]}
     print(json.dumps(line))
 
 
 def reference_wqlinears(torch, model, device, dtype):
-    """One reference-facing module per layer of `model`, sharing the layer's packed buffers: the reference's own
-    WQLinear (staged copy under baseline/_ref, see scripts/stage_reference.py) bound to this repo's plugin, else
-    this repo's mirror of it."""
+    """One reference-facing module per layer of `model`, sharing the layer's packed buffers: this repo's mirror of
+    the reference's WQLinear."""
     import llm_awq_b200 as P
     P.engine()
-    staged = os.path.join(ROOT, "baseline", "_ref")
-    cls, kind = None, "llm_awq_b200.WQLinear (mirror of the reference module)"
-    if os.path.exists(os.path.join(staged, "awq", "quantize", "qmodule.py")):
-        try:
-            if staged not in sys.path:
-                sys.path.insert(0, staged)
-            import contextlib
-            with contextlib.redirect_stdout(sys.stderr):   # the reference prints notices at import: stdout is the JSON line's
-                from awq.quantize.qmodule import WQLinear as RefWQLinear
-            cls, kind = RefWQLinear, "reference awq.quantize.qmodule.WQLinear (unmodified, baseline/_ref) on this plugin"
-        except Exception:  # noqa: BLE001
-            cls = None
     mods = []
     for m in model:
-        if cls is not None:
-            mod = cls(4, G, 128, 8, False, "cpu", dtype=dtype)   # tiny buffers, replaced below
-            mod.in_features, mod.out_features = m["K"], m["N"]
-        else:
-            mod = P.WQLinear(4, G, 128, 8, False, "cpu")
-            mod.in_features, mod.out_features = m["K"], m["N"]
+        mod = P.WQLinear(4, G, 128, 8, False, "cpu")   # tiny buffers, replaced below
+        mod.in_features, mod.out_features = m["K"], m["N"]
         mod.qweight, mod.scales, mod.scaled_zeros = m["qw"], m["sc"], m["sz"]
         mods.append(mod)
-    return mods, kind
+    return mods, "llm_awq_b200.WQLinear (mirror of the reference module)"
 
 
 def tp70b_measure(torch, dist, rank, world, device, steps, warmup):
@@ -626,8 +637,8 @@ def kernel_only_ms(torch, step):
         return None
 
 
-def reference_gpu(torch, model, make_inputs, device, steps, lib=None):
-    """The reference's own CUDA kernels (oracle/_ref: unmodified sources rebuilt for sm_100a) through their own entry
+def reference_gpu(torch, model, make_inputs, device, steps, warmup, lib=None):
+    """The reference's own CUDA kernels (oracle/_ref: unmodified sources rebuilt for sm_90a) through their own entry
     points: plain launches on the legacy default stream (they cannot be graph-captured), and the kernel-only device
     time of the same step.  With `lib`, this repo's C ABI is timed in the SAME two modes beside it."""
     d = os.path.join(ROOT, "oracle", "_ref")
@@ -636,7 +647,7 @@ def reference_gpu(torch, model, make_inputs, device, steps, lib=None):
     ref = importlib.import_module("ref_awq_engine")
     out = {}
     p = lambda t: ctypes.c_void_p(t.data_ptr())
-    for tag, M, k in (("decode", 1, steps), ("prefill", 2048, 5)):
+    for tag, M, k in (("decode", 1, steps), ("prefill", 2048, steps)):
         xs = make_inputs(M, 0.25)
         ys = {N: torch.empty(M, N, dtype=torch.float16, device=device) for N in {m["N"] for m in model}}
 
@@ -655,17 +666,17 @@ def reference_gpu(torch, model, make_inputs, device, steps, lib=None):
                 if rc != 0:
                     raise RuntimeError(lib.b200awq_strerror(rc).decode())
         with torch.cuda.stream(torch.cuda.default_stream()):
-            ms, _ = timed_steps(torch, None, device, step, k, 3)
+            ms, _ = timed_steps(torch, None, device, step, k, warmup)
             ko = kernel_only_ms(torch, step)
         out[tag] = {"value": M * 1000.0 * k / ms, "unit": UNIT, "ms_per_step": ms / k, "steps": k,
                     "eager": {"value": M * 1000.0 * k / ms, "ms_per_step": ms / k},
                     "kernel_only": None if ko is None else {"value": M * 1000.0 / ko, "ms_per_step": ko}}
         if lib is not None:
-            ms_o, _ = timed_steps(torch, None, device, ours, k, 3)
+            ms_o, _ = timed_steps(torch, None, device, ours, k, warmup)
             # kernel-only needs non-overlapping kernels: with programmatic dependent launch a kernel's device duration
             # includes the time it spends prefetching under its predecessor, so the durations are summed with PDL off
             prev = lib.b200awq_set_pdl(0)
-            ms_np, _ = timed_steps(torch, None, device, ours, k, 3)
+            ms_np, _ = timed_steps(torch, None, device, ours, k, warmup)
             ko_o = kernel_only_ms(torch, ours)
             lib.b200awq_set_pdl(prev)
             out[tag]["this_repo_same_modes"] = {
@@ -689,7 +700,7 @@ def run_reference(args):
     pick_cpu_threads(torch, step)
     for _ in range(max(args.warmup, 1)):
         step()
-    steps = min(args.steps, args.cpu_steps)
+    steps = args.steps
     t0 = time.time()
     for _ in range(steps):
         step()
@@ -718,7 +729,7 @@ def run_reference_gpu(args):
     def make_inputs(M, scale=1.0):
         g = torch.Generator(device=device).manual_seed(99 + M)
         return {K: (torch.randn(M, K, generator=g, device=device) * scale).to(torch.float16) for K in (4096, 14336)}
-    r = reference_gpu(torch, model, make_inputs, device, min(args.steps, 200))
+    r = reference_gpu(torch, model, make_inputs, device, args.steps, args.warmup)
     print(json.dumps({"impl": "reference-gpu", "metric": METRIC % 1, "value": r["decode"]["value"], "unit": UNIT, "n_gpus": 1,
                       "higher_is_better": True, "detail": r}))
 
@@ -729,15 +740,14 @@ def main():
     ap.add_argument("--steps", type=int, default=500)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference", "reference-gpu"])
-    ap.add_argument("--prefill-steps", type=int, default=10)
     ap.add_argument("--cpu-seconds", type=float, default=15.0)
-    ap.add_argument("--cpu-steps", type=int, default=30)
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-ref-gpu", dest="ref_gpu", action="store_false")
     ap.add_argument("--no-sweep", dest="sweep", action="store_false")
     ap.add_argument("--workload", default="llama3", choices=["llama3", "tp70b"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32, <= 64 MB in all)")
     args = ap.parse_args()
-    args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     if args.impl == "reference":
         run_reference(args)
     elif args.impl == "reference-gpu":

@@ -1,5 +1,5 @@
 /*
- * b200awq.h — C ABI of the B200-native W4A16 (AWQ v2 layout) quantized-linear path.
+ * b200awq.h — C ABI of the H100-native (sm_90a) W4A16 (AWQ v2 layout) quantized-linear path.
  *
  * This is the drop-in boundary: the two launchers below are what the reference's
  * extension entry points bind to,
@@ -190,7 +190,7 @@ unsigned long long b200awq_launch_count(void);
 /* Human-readable text for a return value of the functions above. */
 const char* b200awq_strerror(int code);
 
-/* "b200awq <version> sm_100a" */
+/* "b200awq <version> sm_90a" */
 const char* b200awq_version(void);
 
 #ifdef __cplusplus

@@ -1,8 +1,8 @@
-"""In-tree build of the sm_100a library and the `awq_inference_engine` extension.
+"""In-tree build of the sm_90a library and the `awq_inference_engine` extension.
 
     python llm_awq_b200/build.py [--force]
 
-Produces (git-ignored, shipped to the GPU box by gpurun):
+Produces (git-ignored build products):
     llm_awq_b200/lib/libb200awq.so                         C ABI (include/b200awq.h), nvcc, no torch
     llm_awq_b200/plugin/awq_inference_engine<EXT>.so       pybind shim over it (g++ + torch headers)
 """
@@ -17,9 +17,9 @@ LIB = os.path.join(HERE, "lib", "libb200awq.so")
 EXT = os.path.join(HERE, "plugin", "awq_inference_engine" + sysconfig.get_config_var("EXT_SUFFIX"))
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
-KERNEL_SRCS = ("api.cu", "w4a16_decode.cu", "w4a16_ring.cu", "w4a16_stream.cu", "w4a16_umma.cu", "w4a16_flat.cu", "rmsnorm.cu", "silu_mul.cu", "attention.cu", "rope_neox.cu")
+KERNEL_SRCS = ("api.cu", "w4a16_decode.cu", "w4a16_ring.cu", "w4a16_stream.cu", "w4a16_wgmma.cu", "rmsnorm.cu", "silu_mul.cu", "attention.cu", "rope_neox.cu")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC"]
 
 
@@ -47,7 +47,7 @@ def build_lib(force=False):
 
 
 def build_trace_lib():
-    """Debug variant with per-launch timestamps (scripts/trace_chain.py); not part of the product."""
+    """Debug variant with per-launch timestamps (-DB200AWQ_TRACE); not part of the product."""
     out = os.path.join(HERE, "lib", "libb200awq_trace.so")
     srcs = [os.path.join(CSRC, f) for f in KERNEL_SRCS]
     _run([os.environ.get("NVCC", "nvcc")] + NVCC_FLAGS + ["-DB200AWQ_TRACE", "-rdc=true", "-shared", "-o", out] + srcs)

@@ -1,5 +1,5 @@
 // C ABI of libb200awq.so (declared in include/b200awq.h): argument validation, dispatch
-// between the HBM-bound streaming kernel and the tcgen05 tensor-core kernel, process-wide
+// between the HBM-bound streaming kernel and the wgmma tensor-core kernel, process-wide
 // switches.  No torch types, no allocation, no synchronisation.
 #include <atomic>
 #include <cstdint>
@@ -26,7 +26,7 @@ struct Config {
   b200awq::DecodeTuning decode_t;
   bool ring;          // B200AWQ_RING=0: never use the persistent ring kernel
   int ring_max_m;     // largest token count served by the ring kernel
-  bool flat;          // B200AWQ_SKINNY=stream: never use the tcgen05 skinny kernel
+  bool flat;          // B200AWQ_SKINNY=stream: never use the wgmma skinny launch
   int flat_min_m, flat_min_m_longk, flat_max_m;
   int stream_max_m;
   b200awq::RingTuning ring_t;
@@ -47,8 +47,8 @@ Config read_config() {
   c.ring_max_m = env_int("B200AWQ_RING_MAX_M", 4);
   const char* sk = std::getenv("B200AWQ_SKINNY");
   c.flat = !(sk && sk[0] == 's');
-  // measured crossovers (profiles/): the tcgen05 skinny kernel from 5 tokens (from 3 when k is long enough to need a
-  // cluster split), the tcgen05 tile kernel above 16
+  // crossovers: the wgmma skinny launch from 5 tokens (from 3 when k is long enough to need a cluster split), the
+  // wgmma tile launch above 16
   c.flat_min_m = env_int("B200AWQ_FLAT_MIN_M", 5);
   c.flat_min_m_longk = env_int("B200AWQ_FLAT_MIN_M", 3);
   c.flat_max_m = env_int("B200AWQ_FLAT_MAX_M", 16);
@@ -100,7 +100,7 @@ int check_device() {
   signed char v = ok[dev].load(std::memory_order_relaxed);
   if (v == 0) {
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-    v = (major == 10) ? 1 : -1;
+    v = (major == 9) ? 1 : -1;
     ok[dev].store(v, std::memory_order_relaxed);
   }
   return v == 1 ? 0 : B200AWQ_ERR_DEVICE;
@@ -290,11 +290,11 @@ int b200awq_w4a16_gemm(const void* x, const void* qweight, const void* scales, c
   if (n % 128) return B200AWQ_ERR_SHAPE;  // reference: N / CTA_N with CTA_N = 128, gemm_cuda.cu:38,1225
   const Config& c = cfg();
   int r = B200AWQ_ERR_SHAPE;
-  // 9..16 tokens on the large layers (>= 48 M weights): the tile kernel (split-k) beats the skinny kernel (measured, call 33
-  // of round 2: 14336 x 4096 at 16 tokens 29.4 vs 37.5 us); everything else below 17 tokens: the small-token kernels
+  // 9..16 tokens on the large layers (>= 48 M weights): the persistent tile launch (split-k); everything else below
+  // 17 tokens: the small-token kernels
   const bool big_mid = m > 8 && (long long)n * k >= 48ll * 1000 * 1000;
   if (m <= 16 && !big_mid) r = launch_small(c, x, qweight, scales, szeros, y, m, n, k, dtype, static_cast<cudaStream_t>(stream));
-  if (r == B200AWQ_ERR_SHAPE)  // 128-channel tcgen05 tiles; split-k over a cluster for small token counts
+  if (r == B200AWQ_ERR_SHAPE)  // 128-channel wgmma tiles; split-k over a cluster for small token counts
     r = b200awq::launch_umma(x, qweight, scales, szeros, y, m, n, k, dtype, pdl_enabled(), c.umma_t,
                              static_cast<cudaStream_t>(stream));
   if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
@@ -335,12 +335,12 @@ const char* b200awq_strerror(int code) {
     case B200AWQ_ERR_BATCH: return "unsupported batch size for gemv kernel (1..7)";
     case B200AWQ_ERR_WORKSPACE: return "workspace too small";
     case B200AWQ_ERR_DRIVER: return "cuTensorMapEncodeTiled unavailable or failed";
-    case B200AWQ_ERR_DEVICE: return "device is not compute capability 10.x (sm_100a kernels only)";
+    case B200AWQ_ERR_DEVICE: return "device is not compute capability 9.x (sm_90a kernels only)";
     case B200AWQ_ERR_PEERS: return "bad peer description for the fused all-reduce";
     default: return code > 0 ? cudaGetErrorString(static_cast<cudaError_t>(code)) : "unknown error";
   }
 }
 
-const char* b200awq_version(void) { return "b200awq 0.1 sm_100a"; }
+const char* b200awq_version(void) { return "b200awq 0.1 sm_90a"; }
 
 }  // extern "C"

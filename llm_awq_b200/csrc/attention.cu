@@ -10,7 +10,7 @@
 //      k, v are written to the cache at slot tlength % L                                   (:1148-1175, :1424-1440)
 //      out = softmax(q . K^T / sqrt(D)) V over positions max(0, tlength + 1 - L) .. tlength  (:1177-1500), fp32 math
 //    ALiBi slopes and fp32 tensors are not supported here (Llama-family callers pass None / fp16, bf16).
-//    B200 design: the G = H / Hkv query heads that share a KV head are served by ONE CTA (the KV bytes are read once,
+//    Design: the G = H / Hkv query heads that share a KV head are served by ONE CTA (the KV bytes are read once,
 //    16-byte loads: K coalesces over positions, V over channels), and long contexts are SPLIT over CTAs (flash-decoding):
 //    every CTA writes (max, sum, unnormalised output) of its chunk to the workspace, the last one to arrive combines.
 //    HBM-bound: algorithmic bytes = 2 * n_pos * D * sizeof(T) per KV head.
@@ -372,7 +372,7 @@ int launch_single_query_attention(const void* q, const void* k, const void* v, v
   a.inv_sqrt_d = 1.f / sqrtf((float)head_dim);
   // worst-case positions (length_per_sample is on the device): the chunking must cover up to min(timestep, max_len - 1) + 1
   const int npos_max = std::min(length_per_sample ? max_len : timestep + 1, max_len);
-  int dev = 0, nsm = 148;
+  int dev = 0, nsm = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
   const int chunk_cap = std::max(256, (48 * 1024 / 4) / G / 32 * 32);  // logits of a chunk: G * chunk floats <= 48 KB
   int splits = std::max(1, std::min(64, 2 * nsm / std::max(1, batch * kv_heads)));

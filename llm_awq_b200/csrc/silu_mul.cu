@@ -46,7 +46,7 @@ __global__ void __launch_bounds__(256) silu_mul_kernel(const T* __restrict__ gat
 
 int launch_silu_mul(const void* gate, const void* up, void* out, size_t count, int dtype, bool pdl, cudaStream_t stream) {
   if (count == 0) return 0;
-  int dev = 0, nsm = 148;
+  int dev = 0, nsm = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
   const size_t want = (count / 8 + 255) / 256;
   cudaLaunchConfig_t cfg{};

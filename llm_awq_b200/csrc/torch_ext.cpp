@@ -240,7 +240,7 @@ void rotary_embedding_neox(at::Tensor& positions, at::Tensor& query, at::Tensor&
 }
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "B200-native drop-in for llm-awq's awq_inference_engine (W4A16 path only)";
+  m.doc() = "H100 (sm_90a) drop-in for llm-awq's awq_inference_engine (W4A16 path only)";
   m.def("gemm_forward_cuda_new", &gemm_forward_cuda_new, "New quantized GEMM kernel.");
   m.def("gemv_forward_cuda_new", &gemv_forward_cuda_new, "New quantized GEMV kernel.");
   m.def("layernorm_forward_cuda", &layernorm_forward_cuda, "FasterTransformer layernorm kernel");

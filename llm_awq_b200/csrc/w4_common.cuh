@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a W4A16 kernels: packed-format index math,
+// Shared device helpers for the sm_90a W4A16 kernels: packed-format index math,
 // exact int4 -> fp16/bf16 dequantisation, mbarrier / bulk-copy / PDL / cluster PTX.
 //
 // Packed format (closed form of the reference packer awq/quantize/qmodule.py:26-65):

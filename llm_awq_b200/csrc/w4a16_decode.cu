@@ -1,20 +1,19 @@
 // One-token W4A16 decode kernel (GEMV, M = 1): the HBM-bound hot path of BASELINE configs[1].
 //
 // Replaces the reference's gemv_kernel (quantization_new/gemv/gemv_cuda.cu:74-229).  Third generation of the decode
-// path; sized from the round-2 measurements (profiles/r2_hbm_probe.txt, profiles/r2_ring_timeline.txt):
-//   * one B200 streams a read-only buffer at 7.2 TB/s through ANY load path provided >= 64 KB per SM are in flight,
-//     but a bulk-async copy (UBLKCP) is worth ~730 ns of latency whatever its size: 4 KB copies with 20 KB in flight
-//     stop at 4.2 TB/s (the second-generation ring of w4a16_ring.cu moved 4 KB copies: its streaming limit with the
-//     math switched off was 3.7 TB/s).  Here every copy is one QUAD ROW (4 output channels, contiguous over k in the
-//     packed layout) x up to 4096 input channels = 8 KB, and 70..88 KB of copies are in flight per CTA.
-//   * a launch boundary costs ~2 us in which nothing can be computed (the previous layer's tail, ~1 us for
-//     griddepcontrol.wait to return, the staging of the activations).  Two CTAs of consecutive launches co-reside on
+// path:
+//   * HBM streams a read-only buffer at full rate only with tens of KB in flight per SM, and a bulk-async copy
+//     (UBLKCP) carries a fixed latency whatever its size, so small copies cap the rate.  Here every copy is one QUAD
+//     ROW (4 output channels, contiguous over k in the packed layout) x up to 4096 input channels = 8 KB, and
+//     70..88 KB of copies are in flight per CTA.
+//   * a launch boundary costs microseconds in which nothing can be computed (the previous layer's tail,
+//     griddepcontrol.wait, the staging of the activations).  Two CTAs of consecutive launches co-reside on
 //     every SM (<= 113 KB and <= 102 registers x 320 threads each), the PRODUCER warp never waits for the activations,
 //     so HBM keeps streaming into the next launch's ring through the bubble; the consumers then have to drain the ring
 //     faster than HBM fills it: int8 tensor-core MACs on the packed bytes AS THEY ARE (no dequantisation).
 //
 // Work split: the N / 4 quad rows are dealt evenly and contiguously to the clusters (S CTAs each, S = 1 unless the
-// layer has too few rows to balance 148 SMs, then k is split S ways inside the cluster and rank 0 adds the partial
+// layer has too few rows to balance the SMs, then k is split S ways inside the cluster and rank 0 adds the partial
 // sums it receives through distributed shared memory).  A CTA walks its quad rows in ROW BLOCKS of 16 channels (4
 // quad rows; the last block may hold fewer) and, for long k, in PIECES of <= 32 groups of 128 input channels.
 //

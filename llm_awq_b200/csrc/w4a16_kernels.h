@@ -31,7 +31,7 @@ struct StreamTuning {
 };
 
 struct UmmaTuning {
-  int tn = 0;      // 0 = auto, else token tile (32 / 64 / 128 / 256)   [env B200AWQ_UMMA_TN]
+  int tn = 0;      // 0 = auto, else token tile (16 / 32 / 64 / 128)    [env B200AWQ_UMMA_TN]
   int max_ctas = 0;  // 0 = one per SM                                   [env B200AWQ_UMMA_CTAS]
   int split = 0;     // 0 = auto, 1 = never, 2/4/8 = split k over a cluster [env B200AWQ_UMMA_SPLIT]
 };
@@ -54,7 +54,7 @@ struct FlatTuning {
 int launch_stream(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
                   bool pdl, const StreamTuning& tune, cudaStream_t stream, const PeerArgs* peers = nullptr);
 
-// tcgen05 / TMA / TMEM tensor-core kernel, any M (w4a16_umma.cu)
+// TMA + wgmma tensor-core kernel, any M, N % 128 == 0 (w4a16_wgmma.cu)
 int launch_umma(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
                 bool pdl, const UmmaTuning& tune, cudaStream_t stream);
 
@@ -101,7 +101,7 @@ int launch_rope_neox(const long long* positions, void* query, void* key, const v
                      int k_heads, int head_size, int rot_dim, long long q_stride, long long k_stride, int dtype, bool pdl,
                      cudaStream_t stream);
 
-// tcgen05 skinny-batch kernel, 1 <= M <= 64, N % 128 == 0 (w4a16_flat.cu)
+// the same kernel for skinny batches, 1 <= M <= 64, N % 128 == 0: one CTA per tile and k slice (w4a16_wgmma.cu)
 int launch_flat(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
                 bool pdl, const FlatTuning& tune, cudaStream_t stream);
 

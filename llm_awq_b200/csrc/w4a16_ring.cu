@@ -2,8 +2,7 @@
 // fp16 / bf16 tensor-core MACs with the tokens in the MMA columns.  (One fp16 token is served by w4a16_decode.cu, the
 // third generation of this structure: 8 KB copies instead of the 4 KB ones below, int8-digit MACs.)
 //
-// Replaces the reference's gemv_kernel (quantization_new/gemv/gemv_cuda.cu:74-229).  B200-first design, sized
-// from the round-1 measurements (profiles/README.md, "What limits decode"):
+// Replaces the reference's gemv_kernel (quantization_new/gemv/gemv_cuda.cu:74-229).  Design:
 //   * ONE CTA per SM per launch (grid = #SMs), ~95 KB of shared memory and <= 102 registers per thread, so the
 //     CTAs of TWO consecutive launches co-reside on every SM: with programmatic dependent launch the next
 //     layer's CTA fills its whole ring with weights while this layer is still computing.  No CTA churn: the
@@ -15,8 +14,8 @@
 //     The producer never waits for the activations, so it runs ahead of griddepcontrol.wait.
 //   * 8 CONSUMER warps split the slot's 16 groups of 128 input channels.  Quad rows are placed 4 KB + 16 B
 //     apart, which makes the eight 16-byte rows of every ldmatrix phase hit eight different bank groups: the
-//     packed words go shared -> registers with ldmatrix.x4 at full shared-memory bandwidth (the round-1 kernel
-//     had 2-way conflicts on every weight read).  ldmatrix hands lane (g, tig) word `tig` of the chunk
+//     packed words go shared -> registers with ldmatrix.x4 at full shared-memory bandwidth (a plain layout
+//     has 2-way conflicts on every weight read).  ldmatrix hands lane (g, tig) word `tig` of the chunk
 //     (channel g, 32-k block m) for m = 0..3; one LOP3 per nibble pair turns it into the A operand of
 //     m16n8k16 tensor-core MACs (rows = 16 channels, columns = tokens, fp32 accumulate).  The activations are
 //     staged ONCE per CTA in the matching order, so every B fragment is an aligned register pair.

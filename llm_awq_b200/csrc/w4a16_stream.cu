@@ -1,7 +1,7 @@
 // HBM-bound W4A16 streaming kernel for small token counts (decode GEMV, M <= 16).
 //
 // Replaces the reference's gemv_kernel (quantization_new/gemv/gemv_cuda.cu:74-229) and,
-// for 8 <= M <= 16, its split-K GEMM tile (gemm_cuda.cu:1155-1168).  Design (B200-first):
+// for 8 <= M <= 16, its split-K GEMM tile (gemm_cuda.cu:1155-1168).  Design:
 //   * one CTA owns 8*RO output channels x Kc input channels.  Its slice of `qweight`
 //     is 2*RO contiguous byte ranges (the packing interleaves 4 rows, so a 4-row "quad"
 //     is contiguous over k); they are pulled into shared memory with bulk async copies
@@ -57,8 +57,8 @@ constexpr unsigned long long kExchangeTimeoutNs = 10ull * 1000 * 1000 * 1000;
 __device__ unsigned int g_exchange_dead = 0;
 
 #ifdef B200AWQ_TRACE
-// Debug build only (scripts/trace_chain.py): wall-clock stamps of the first and last CTA of each launch.
-__device__ unsigned long long g_trace_buf[1024 * 2 * 8];  // shared with w4a16_flat.cu (needs -rdc)
+// Debug build only (-DB200AWQ_TRACE): wall-clock stamps of the first and last CTA of each launch.
+__device__ unsigned long long g_trace_buf[1024 * 2 * 8];
 #define B200AWQ_STAMP(ev)                                                     \
   if (threadIdx.x == 0 && (blockIdx.x == 0 || blockIdx.x == gridDim.x - 1)) \
   g_trace_buf[(((unsigned)seq & 1023u) * 2 + (blockIdx.x != 0)) * 8 + (ev)] = globaltimer_ns()
@@ -503,7 +503,7 @@ static int launch_stream_w(const void* x, const void* qw, const void* sc, const 
   if (pa.world > 1 && TT != 1) return B200AWQ_ERR_SHAPE;
   // several row blocks per CTA (all weight slices prefetched up front, activations / group sums staged once) is a
   // tuning knob only: fat long-lived CTAs keep the NEXT launch's CTAs from becoming resident, which costs more
-  // than the saved prologues (measured, profiles/README.md)
+  // than the saved prologues
   const int nblk = N / (8 * RO);
   int rbs = (tune.rbs > 0) ? tune.rbs : 1;
   if (S != 1 || rbs > nblk) rbs = 1;
@@ -521,7 +521,11 @@ static int launch_stream_w(const void* x, const void* qw, const void* sc, const 
   // CTAs only need enough room to prefetch); multi-wave launches want as many as fit (measured, DESIGN.md).
   size_t dyn = L.total;
   const int ctas = ((nblk + rbs - 1) / rbs) * S;
-  const int per_sm = ctas <= 2 * 148 ? 2 : (ctas <= 3 * 148 ? 3 : 0);
+  int dev = 0, nsm = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+  if (nsm <= 0) nsm = 132;
+  const int per_sm = ctas <= 2 * nsm ? 2 : (ctas <= 3 * nsm ? 3 : 0);
   if (tune.pad > 0)  // > 0: explicit extra bytes (limits co-residency), 0: heuristic, < 0: none
     dyn += (size_t)tune.pad;
   else if (tune.pad == 0 && per_sm > 0 && S == 1)
@@ -554,7 +558,7 @@ template <typename T, int RO, int TT, int MODE>
 static int launch_stream_t(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K,
                            int S, int rpb, bool pdl, const StreamTuning& tune, cudaStream_t stream, const PeerArgs* peers) {
   // 8 warps per CTA by default; 16 (shorter serial chain after griddepcontrol.wait, half the co-residency) is a knob
-  if (tune.warps == 16)  // measured (profiles/): 16 warps or several row blocks per CTA do not pay
+  if (tune.warps == 16)  // 16 warps or several row blocks per CTA do not pay
     return launch_stream_w<T, RO, TT, MODE, 16>(x, qw, sc, sz, y, M, N, K, S, rpb, pdl, tune, stream, peers);
   return launch_stream_w<T, RO, TT, MODE, 8>(x, qw, sc, sz, y, M, N, K, S, rpb, pdl, tune, stream, peers);
 }
@@ -576,7 +580,7 @@ int launch_stream(const void* x, const void* qw, const void* sc, const void* sz,
   if (M < 1 || M > 16 || N % 8 || K % kGroup) return B200AWQ_ERR_SHAPE;
   const int ro = (N % 16 == 0) ? 2 : 1;
   // k per CTA: splitting k over a cluster doubles the CTAs and adds the cluster reduction; up to 4 tokens the unsplit
-  // 4096 measured 1.1-1.5x faster than 2048 (profiles/README.md, batch sweep), above that shared memory for x decides
+  // 4096 rather than 2048, above that shared memory for x decides
   const int kc_target = M <= 4 ? 4096 : (M <= 8 ? 2048 : 1024);
   const int S = pick_splits(K, kc_target, tune.kc);
   const int rpb = tune.rpb > 0 ? tune.rpb : 64;  // default: one barrier (4 large copies) per CTA

@@ -1,4 +1,4 @@
-"""Locate and load the built sm_100a artefacts.  There is NO fallback: if the library or
+"""Locate and load the built sm_90a artefacts.  There is NO fallback: if the library or
 the extension is missing (or there is no CUDA device when a kernel is called) this raises."""
 import ctypes
 import importlib

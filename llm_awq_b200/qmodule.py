@@ -5,7 +5,7 @@ the same dispatch rule as awq/quantize/qmodule.py (WQLinear :78-235, pack_intwei
 :26-65, calculate_zeros_width :11-23), so state dicts (`qweight`, `scales`,
 `scaled_zeros`, `bias`) are interchangeable and the parity tests read like the
 reference's call sites.  The packer is a closed-form, vectorised restatement (no
-per-column Python loop); the forward pass calls the sm_100a kernels through the
+per-column Python loop); the forward pass calls the sm_90a kernels through the
 `awq_inference_engine` extension and nothing else — there is no CPU or PyTorch fallback.
 """
 import torch

@@ -11,8 +11,8 @@ Why slicing the packed tensors is legal (closed form of pack_intweight, qmodule.
     - a row-parallel (input-channel) shard is a contiguous block of int16 COLUMNS of `qweight`
       at 64-granularity; scales/zeros rows follow at group (128) granularity and are re-padded
       to a multiple of 8 rows like calculate_zeros_width does (qmodule.py:11-23).
-One process per GPU; the collective is torch.distributed (NCCL over NVLink on the GPU box, gloo in
-the CPU tests).  The local product is always the sm_100a kernel: there is no CPU fallback.
+One process per GPU; the collective is torch.distributed (NCCL over NVLink on GPUs, gloo in
+the CPU tests).  The local product is always the sm_90a kernel: there is no CPU fallback.
 """
 import torch
 import torch.nn as nn

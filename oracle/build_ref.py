@@ -1,13 +1,14 @@
-"""Build oracle/_ref/ref_awq_engine*.so: the REFERENCE's own W4A16 kernels for sm_100a.
+"""Build oracle/_ref/ref_awq_engine*.so: the REFERENCE's own W4A16 kernels for sm_90a.
 
 Compiles awq/kernels/csrc/quantization_new/{gemv/gemv_cuda.cu,gemm/gemm_cuda.cu}, layernorm/layernorm.cu and
 position_embedding/pos_encoding_kernels.cu from
-where they lie under /root/reference (nothing is copied into this repo) with the
-reference's nvcc flags (awq/kernels/setup.py:7-21) plus an explicit sm_100a gencode,
-and links them with oracle/ref_binding.cpp.  Output goes to oracle/_ref/ (git-ignored,
-but it travels to the GPU box with gpurun).  Does not run the reference's setup.py.
+an llm-awq checkout named by $AWQ_REFERENCE (nothing is copied into this repo) with the
+reference's nvcc flags (awq/kernels/setup.py:7-21) plus an explicit sm_90a gencode,
+and links them with oracle/ref_binding.cpp.  Output goes to oracle/_ref/ (git-ignored).
+Does not run the reference's setup.py.  The GPU tests do not need it: they compare with
+the reference outputs stored under tests/golden/ (tests/golden/make_ref_kernel_golden.py).
 
-Usage: python oracle/build_ref.py     (about 5 minutes; skipped if up to date)
+Usage: AWQ_REFERENCE=<llm-awq checkout> python oracle/build_ref.py     (about 5 minutes; skipped if up to date)
 """
 import os
 import subprocess
@@ -16,7 +17,7 @@ import sysconfig
 from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = os.environ.get("AWQ_REFERENCE", "/root/reference")
+REF = os.environ.get("AWQ_REFERENCE", "")
 CSRC = os.path.join(REF, "awq/kernels/csrc")
 OUT = os.path.join(HERE, "_ref")
 EXT = sysconfig.get_config_var("EXT_SUFFIX")
@@ -24,7 +25,7 @@ TARGET = os.path.join(OUT, "ref_awq_engine" + EXT)
 
 
 def available() -> bool:
-    return os.path.isdir(CSRC)
+    return bool(REF) and os.path.isdir(CSRC)
 
 
 def build(force: bool = False) -> str | None:
@@ -43,7 +44,7 @@ def build(force: bool = False) -> str | None:
     inc = [f"-I{p}" for p in ce.include_paths("cuda")] + [f"-I{sysconfig.get_paths()['include']}", f"-I{CSRC}"]
     common = ["-DTORCH_EXTENSION_NAME=ref_awq_engine", "-DTORCH_API_INCLUDE_EXTENSION_H",
               "-D_GLIBCXX_USE_CXX11_ABI=1", "-DENABLE_BF16"]
-    nvcc = ["nvcc", "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a",
+    nvcc = ["nvcc", "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a",
             "-U__CUDA_NO_HALF_OPERATORS__", "-U__CUDA_NO_HALF_CONVERSIONS__",
             "-U__CUDA_NO_BFLOAT16_OPERATORS__", "-U__CUDA_NO_BFLOAT16_CONVERSIONS__",
             "-U__CUDA_NO_BFLOAT162_OPERATORS__", "-U__CUDA_NO_BFLOAT162_CONVERSIONS__",

@@ -6,14 +6,14 @@ this file.
 Parity status: the reference has no tests or golden vectors for these ops and its kernels are CUDA-only.  The
 restatements below are pinned twice:
   * on CPU (``tests/test_layer_oracle_golden.py``) against fixtures produced by the reference's own PYTHON definitions
-    of the same ops, imported in the build container by ``tests/golden/make_golden.py::layer_ops_golden`` ->
+    of the same ops, imported on the CPU by ``tests/golden/make_golden.py::layer_ops_golden`` ->
     ``tests/golden/reference_layer_ops.npz``: ``RMSNorm._norm`` (tinychat/models/llama.py:24-31),
     ``precompute_freqs_cis`` + ``apply_rotary_emb`` (:39-47, :68-84), ``precompute_freqs`` (:50-57: the table
     ``fused_rope_with_pos`` consumes), and the KV-cache store + softmax attention of the prefill branch
     (tinychat/modules/fused_attn.py:256-305) whose last row a decode step must reproduce; ``mlp_front`` against the
     reference's unmodified ``QuantLlamaMLP.our_llama_mlp`` EXECUTED on CPU over oracle-backed engine calls
     (``make_golden.py::mlp_callsite_golden`` -> ``tests/golden/reference_mlp_callsite.npz``);
-  * on the GPU box against the reference's own kernels recompiled for sm_100a (``oracle/_ref``:
+  * on the GPU against the reference's own kernels' outputs stored under ``tests/golden/`` (``oracle/_ref``:
     ``layernorm_forward_cuda``) and, for the fused MLP front half, against the composition the reference executes
     (two engine calls + ``F.silu`` + multiply, ``tinychat/modules/fused_mlp.py:36-83``) evaluated with torch.
 The reference's attention KERNEL (FasterTransformer template) is not rebuilt (DESIGN.md §4).

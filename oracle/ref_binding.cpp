@@ -1,7 +1,7 @@
 // Our own 4-function binding around the REFERENCE's W4A16 kernels (compiled from where
-// they lie under /root/reference by oracle/build_ref.py; sources are never copied).
+// they lie in the checkout named by $AWQ_REFERENCE by oracle/build_ref.py; sources are never copied).
 // Module name: ref_awq_engine.  Test infrastructure only (GPU-side parity oracle and the
-// "reference-on-B200" timing column).
+// "reference_on_gpu" timing column of bench.py).
 #include <torch/extension.h>
 #include "quantization_new/gemm/gemm_cuda.h"   // reference: gemm_forward_cuda_new
 #include "quantization_new/gemv/gemv_cuda.h"   // reference: gemv_forward_cuda_new

@@ -7,10 +7,10 @@ TEST INFRASTRUCTURE ONLY.  Nothing under ``llm_awq_b200/`` may import this file;
 Parity status: the reference ships no tests or golden vectors for this path
 (SURVEY.md §4), so it is *pinned by us*: every function below is checked against the
 reference's own Python (``awq/quantize/qmodule.py``, ``awq/quantize/quantizer.py``)
-imported on CPU in the build container; the resulting vectors are committed under
+imported on CPU; the resulting vectors are committed under
 ``tests/golden/`` together with ``tests/golden/make_golden.py``.  The CUDA kernels of
-the reference cannot run in the build container (no GPU); on the GPU box the parity
-tests additionally compare against the reference kernels recompiled for sm_100a
+the reference's kernels need a GPU; on the GPU the parity
+tests additionally compare against stored outputs of the reference kernels built for sm_90a
 (``oracle/_ref``, built by ``oracle/build_ref.py``).
 
 Each function cites the reference file:line it restates (paths relative to the

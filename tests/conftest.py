@@ -9,8 +9,8 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
-    config.addinivalue_line("markers", "multigpu: needs at least 2 CUDA devices (gpurun --gpus 2); deselected elsewhere")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (sm_90a)")
+    config.addinivalue_line("markers", "multigpu: needs at least 2 CUDA devices; skipped elsewhere")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -20,13 +20,13 @@ def pytest_collection_modifyitems(config, items):
     except Exception:
         has_gpu = False
     if has_gpu:
-        # tests that need several GPUs are DESELECTED (not skipped) on a single-GPU box: the 1-GPU suite reports 0 skips,
-        # their single-GPU stand-ins are tests/test_tp_loopback_gpu.py
+        # tests that need several GPUs skip on a single-GPU machine; their single-GPU stand-ins are
+        # tests/test_tp_loopback_gpu.py
         if torch.cuda.device_count() < 2:
-            multi = [i for i in items if "multigpu" in i.keywords]
-            if multi:
-                config.hook.pytest_deselected(items=multi)
-                items[:] = [i for i in items if "multigpu" not in i.keywords]
+            multi = pytest.mark.skip(reason="needs at least 2 CUDA devices")
+            for item in items:
+                if "multigpu" in item.keywords:
+                    item.add_marker(multi)
         return
     skip = pytest.mark.skip(reason="no CUDA device in this container")
     for item in items:

@@ -1,8 +1,8 @@
 """Generate tests/golden/*.npz by running the REFERENCE's own Python on CPU.
 
-Run in the build container only (needs /root/reference; the GPU box does not have it):
+Needs an llm-awq checkout named by $AWQ_REFERENCE:
 
-    python tests/golden/make_golden.py
+    AWQ_REFERENCE=<llm-awq checkout> python tests/golden/make_golden.py
 
 The reference module ``awq.quantize.qmodule`` does ``import awq_inference_engine`` at
 import time (qmodule.py:4); a stub module is registered for that name because only the
@@ -17,7 +17,7 @@ import types
 import numpy as np
 import torch
 
-REF = os.environ.get("AWQ_REFERENCE", "/root/reference")
+REF = os.environ["AWQ_REFERENCE"]
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 

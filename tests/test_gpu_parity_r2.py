@@ -1,4 +1,4 @@
-"""Round-2 parity cases (VERDICT r1, "parity holes"): Llama-2-70B TP=1 / TP=8-shard shapes over the whole
+"""Further parity cases: Llama-2-70B TP=1 / TP=8-shard shapes over the whole
 token sweep, the two known-answer tests SURVEY.md §8c(5) lists (all-ones weights, single non-zero group), the
 persistent ring kernel's partition edge cases, and its determinism."""
 import ctypes
@@ -86,7 +86,7 @@ def test_kat_single_nonzero_group(M, grp, dtype):
 @pytest.mark.parametrize("N,K", [(8, 2048), (16, 4096), (1184, 2048), (1192, 2176), (2376, 4224), (4744, 2048),
                                  (296, 6144), (8, 128), (40, 1920)])
 def test_ring_partition_edges(N, K, M, dtype):
-    """Channel counts around multiples of the SM count (148 CTAs, 74 clusters: fewer octets than clusters, exactly
+    """Channel counts around multiples of an SM count (148 CTAs, 74 clusters: fewer octets than clusters, exactly
     one / two per cluster, an odd octet at the end), odd group counts (k split 8|9, 16|17), k below the split
     threshold, slots of fewer than 16 groups."""
     qw, s, z = gen_layer(N, K, dtype, seed=N + K, device=DEV)

@@ -1,7 +1,7 @@
 """Tensor-parallel sharding in packed space (llm_awq_b200/tp.py): shard algebra against the oracle,
 and the row-parallel all-reduce path with world_size 2 and 4 gloo processes on CPU.  The local product in
 the CPU processes is the ORACLE standing in for the kernel (test harness only — the product module has
-no CPU path; on the GPU box tests/test_gpu_parity.py::test_tp_* run the same modules on the kernels)."""
+no CPU path; on the GPU tests/test_gpu_parity.py::test_tp_* run the same modules on the kernels)."""
 import os
 
 import numpy as np

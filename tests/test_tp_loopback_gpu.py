@@ -3,7 +3,7 @@ include/b200awq.h): the `world` ranks are `world` launches on `world` streams of
 exchange buffer (plain device memory instead of NVLink peer mappings) and its own k-slice of the layer.  The protocol
 is exactly the multi-GPU one -- every rank stores its fp32 partials with the call's epoch into every peer's buffer
 and polls its own -- so world = 2, 4 and 8, several token counts, repeated calls (epoch advance), layers of different
-widths sharing one exchange are all exercised on the 1-GPU test box (VERDICT r1, item 2b; the real NVLink run, incl.
+widths sharing one exchange are all exercised on one GPU (the real NVLink run, incl.
 CUDA-graph replay, is tests/test_tp_gpu.py -- a graph's branches are not GUARANTEED to run concurrently on one device,
 and ranks that wait for each other must be).
 
