@@ -44,7 +44,7 @@ extern "C" {
 #define B200AWQ_DTYPE_BF16 1
 
 #define B200AWQ_OK 0
-#define B200AWQ_ERR_SHAPE (-1)     /* n % 8 (gemv) / n % 128 (gemm), k % 128, m out of range */
+#define B200AWQ_ERR_SHAPE (-1)     /* n % 8 (gemv) / n % 128 (gemm), k % 128 (w8a8: k % 16), m out of range */
 #define B200AWQ_ERR_GROUP (-2)     /* group_size != 128 (reference: gemv_cuda.cu:289,332-335) */
 #define B200AWQ_ERR_ALIGN (-3)     /* a pointer is NULL or not 16-byte aligned */
 #define B200AWQ_ERR_DTYPE (-4)     /* dtype is not F16 / BF16 (reference: dispatch_utils.cuh:7-18) */
@@ -166,6 +166,49 @@ int b200awq_rope_with_pos(const void* x, const float* freqs, void* y, int s, int
 int b200awq_rotary_embedding_neox(const long long* positions, void* query, void* key, const void* cos_sin_cache, int tokens,
                                   int q_heads, int k_heads, int head_size, int rot_dim, long long q_token_stride,
                                   long long k_token_stride, int dtype, void* stream);
+
+/* ---- W8A8 (int8 weights, int8 per-token activations): the vision-tower ops of the reference's extension
+ * (csrc/pybind.cpp:30-37), called by awq/quantize/w8a8_linear.py and tinychat's QuantSiglipEncoder /
+ * QuantInternVisionEncoder.  Scales are fp16 everywhere (the reference reads them as at::Half).  fp32 activations,
+ * which the reference also dispatches, are rejected with B200AWQ_ERR_DTYPE.  The row ops take rows of at most
+ * 32768 elements, 8192 when n % 8 != 0 or a row pointer is not 16-byte aligned (B200AWQ_ERR_SHAPE beyond); m == 0
+ * is a no-op. */
+
+/* y[i, j] = rn_f16(f32(acc) * (wscales[j] * ascales[i]))                    bias == NULL
+ *         = rn_f16(fma(ascales[i], f32(acc) * wscales[j], bias[j]))         otherwise
+ * with acc = sum_k x[i, k] w[j, k] exact in int32, every fp32 product flushing denormals.  Replaces
+ *   w8a8_gemm_forward_cuda(in_feats, kernel, wscales, ascales, out_feats)             w8a8/w8a8_gemm_cuda.cu:907-953
+ *   w8a8_gemm_fuse_bias_forward_cuda(in_feats, kernel, wscales, ascales, out, bias)   w8a8/w8a8_gemm_cuda.cu:586-633
+ * x [m, k] int8, w [n, k] int8 (the plain [OC, IC] matrix of W8A8OF16LinearDynamicInputScale, not repacked), both
+ * row-major and 16-byte aligned; wscales [n], ascales [m], bias [n] fp16; y [m, n] fp16, 16-byte aligned.
+ * m >= 1, n % 8 == 0, k % 16 == 0 (any k tail is exact). */
+int b200awq_w8a8_gemm(const void* x, const void* w, const void* wscales, const void* ascales, const void* bias, void* y,
+                      int m, int n, int k, void* stream);
+
+/* Per-token int8 quantisation: scales[i] = rn_f16(amax_i / 127), q[i, j] = cvt.rni.sat(x[i, j] * (127 / amax_i)),
+ * amax_i = max_j |x[i, j]| (a zero row gives codes 0 and scale 0).  Replaces invoke_quant(out, input, scale),
+ * w8a8/quantization.cu:54-112.  x [m, n] of dtype, q [m, n] int8, scales [m] fp16. */
+int b200awq_quant_per_token(const void* x, void* q, void* scales, int m, int n, int dtype, void* stream);
+
+/* LayerNorm + int8 quantisation.  Replaces rms_norm_general(out, input, weight, bias, scaling, epsilon,
+ * use_per_token_quant), w8a8/layernorm.cu:55-231 -- a LayerNorm (mean, E[x^2] - E[x]^2, rsqrt) despite the name.
+ *   per_token != 0: y = (x - mean) rstd gamma + beta (beta may be NULL); amax over rn_T(y) starting from 1e-6;
+ *                   q = cvt.rni.sat(y * (127 / amax)) from the unrounded y; scale[i] = rn_f16(amax / 127)  [m]
+ *   per_token == 0: the reference's per-tensor branch: beta is IGNORED and q = cvt.rni.sat(rn_T(y) * scale[0])
+ *                   (scale[0] multiplies); scale is read, not written.
+ * x [m, n], gamma / beta [n] of dtype, q [m, n] int8. */
+int b200awq_layernorm_quant(const void* x, const void* gamma, const void* beta, void* q, void* scale, int m, int n,
+                            float eps, int per_token, int dtype, void* stream);
+
+/* GELU (tanh form, the reference's fp16 operation chain around tanh.approx) + per-token int8 quantisation, fp16 only
+ * like the reference.  tmp[i, j] = gelu(x[i, j]); amax_i over |tmp| except values in (0, 1e-4], which enter negated;
+ * scales[i] = rn_f16(amax_i / 127); q = cvt.rni.sat(f32(rn_f16(rn_f16(127 / amax_i) * tmp))).  Replaces
+ * gelu_and_quant(out, input, scale_out, tmp), w8a8/act.cu:22-96.  x, tmp [m, n] fp16, q [m, n] int8, scales [m]. */
+int b200awq_gelu_quant(const void* x, void* q, void* scales, void* tmp, int m, int n, void* stream);
+
+/* y[i, j] = rn_T(rn_T(silu(x[i, j])) * x[i, d + j]) for x [m, 2d], y [m, d] of dtype.  Replaces
+ * silu_and_mul(input), w8a8/act.cu:107-140 (same kernel as the MLP front half's tail, with a row pitch). */
+int b200awq_silu_and_mul(const void* x, void* y, int m, int d, int dtype, void* stream);
 
 /* Names used by BASELINE.json's north_star; identical to the two launchers above. */
 int gemv_forward_4bit(const void* x, const void* qweight, const void* scales, const void* szeros,

@@ -17,7 +17,8 @@ LIB = os.path.join(HERE, "lib", "libb200awq.so")
 EXT = os.path.join(HERE, "plugin", "awq_inference_engine" + sysconfig.get_config_var("EXT_SUFFIX"))
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
-KERNEL_SRCS = ("api.cu", "w4a16_decode.cu", "w4a16_ring.cu", "w4a16_stream.cu", "w4a16_wgmma.cu", "rmsnorm.cu", "silu_mul.cu", "attention.cu", "rope_neox.cu")
+KERNEL_SRCS = ("api.cu", "w4a16_decode.cu", "w4a16_ring.cu", "w4a16_stream.cu", "w4a16_wgmma.cu", "rmsnorm.cu", "silu_mul.cu", "attention.cu", "rope_neox.cu",
+               "w8a8_wgmma.cu", "w8a8_rowops.cu")
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC"]
@@ -36,7 +37,7 @@ def _run(cmd):
 
 def build_lib(force=False):
     srcs = [os.path.join(CSRC, f) for f in KERNEL_SRCS]
-    deps = srcs + [os.path.join(CSRC, f) for f in ("w4_common.cuh", "w4a16_kernels.h", "rope_neox.cuh")] + \
+    deps = srcs + [os.path.join(CSRC, f) for f in ("w4_common.cuh", "w4a16_kernels.h", "rope_neox.cuh", "tma_wgmma.cuh", "w8a8_math.cuh")] + \
         [os.path.join(INCLUDE, "b200awq.h"), __file__]
     if not force and _newer(LIB, deps):
         return LIB

@@ -4,6 +4,7 @@
 #include <atomic>
 #include <cstdint>
 #include <cstdlib>
+#include <initializer_list>
 
 #include "w4a16_kernels.h"
 
@@ -219,7 +220,7 @@ int b200awq_w4a16_mlp_front(const void* x, const void* gate_qweight, const void*
     if (r != 0) return r;
     g_launches.fetch_add(1, std::memory_order_relaxed);
   }
-  const int r = b200awq::launch_silu_mul(g, u, y, (size_t)m * n, dtype, pdl_enabled(), st);
+  const int r = b200awq::launch_silu_mul(g, u, y, 1, (size_t)m * n, (size_t)m * n, dtype, pdl_enabled(), st);
   if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
   return r;
 }
@@ -301,6 +302,66 @@ int b200awq_w4a16_gemm(const void* x, const void* qweight, const void* scales, c
   return r;
 }
 
+// ---------------------------------------------------------------- W8A8
+int b200awq_w8a8_gemm(const void* x, const void* w, const void* wscales, const void* ascales, const void* bias, void* y,
+                      int m, int n, int k, void* stream) {
+  if (m < 1 || n < 8 || k < 16 || n % 8 || k % 16) return B200AWQ_ERR_SHAPE;
+  if (!aligned16(x) || !aligned16(w) || !aligned16(y) || !wscales || !ascales) return B200AWQ_ERR_ALIGN;
+  if ((reinterpret_cast<uintptr_t>(wscales) | reinterpret_cast<uintptr_t>(ascales) | reinterpret_cast<uintptr_t>(bias)) & 1u)
+    return B200AWQ_ERR_ALIGN;
+  if (int e = check_device()) return e;
+  const int r = b200awq::launch_w8a8_gemm(x, w, wscales, ascales, bias, y, m, n, k, pdl_enabled(),
+                                          static_cast<cudaStream_t>(stream));
+  if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
+  return r;
+}
+
+namespace {
+// common checks of the W8A8 row ops: 16-bit activations, rows the kernels hold in registers, non-null 2-byte aligned
+// pointers (the int8 codes are written one byte at a time when not 16-byte aligned, so any even address will do)
+int check_rows(int m, int n, int dtype, std::initializer_list<const void*> ptrs) {
+  if (dtype != B200AWQ_DTYPE_F16 && dtype != B200AWQ_DTYPE_BF16) return B200AWQ_ERR_DTYPE;
+  if (m < 0 || n < 1 || n > b200awq::w8a8_row_limit()) return B200AWQ_ERR_SHAPE;
+  for (const void* p : ptrs)
+    if (!p || (reinterpret_cast<uintptr_t>(p) & 1u)) return B200AWQ_ERR_ALIGN;
+  return check_device();
+}
+int counted(int r, int m) {
+  if (r == 0 && m > 0) g_launches.fetch_add(1, std::memory_order_relaxed);
+  return r;
+}
+}  // namespace
+
+int b200awq_quant_per_token(const void* x, void* q, void* scales, int m, int n, int dtype, void* stream) {
+  if (int e = check_rows(m, n, dtype, {x, scales, q})) return e;
+  return counted(b200awq::launch_quant_per_token(x, q, scales, m, n, dtype, pdl_enabled(), static_cast<cudaStream_t>(stream)), m);
+}
+
+int b200awq_layernorm_quant(const void* x, const void* gamma, const void* beta, void* q, void* scale, int m, int n,
+                            float eps, int per_token, int dtype, void* stream) {
+  if (reinterpret_cast<uintptr_t>(beta) & 1u) return B200AWQ_ERR_ALIGN;
+  if (int e = check_rows(m, n, dtype, {x, gamma, scale, q})) return e;
+  return counted(b200awq::launch_layernorm_quant(x, gamma, beta, q, scale, m, n, eps, per_token != 0, dtype, pdl_enabled(),
+                                                 static_cast<cudaStream_t>(stream)),
+                 m);
+}
+
+int b200awq_gelu_quant(const void* x, void* q, void* scales, void* tmp, int m, int n, void* stream) {
+  if (int e = check_rows(m, n, B200AWQ_DTYPE_F16, {x, scales, tmp, q})) return e;
+  return counted(b200awq::launch_gelu_quant(x, q, scales, tmp, m, n, pdl_enabled(), static_cast<cudaStream_t>(stream)), m);
+}
+
+int b200awq_silu_and_mul(const void* x, void* y, int m, int d, int dtype, void* stream) {
+  if (dtype != B200AWQ_DTYPE_F16 && dtype != B200AWQ_DTYPE_BF16) return B200AWQ_ERR_DTYPE;
+  if (m < 0 || d < 1) return B200AWQ_ERR_SHAPE;
+  if (!x || !y || ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 1u)) return B200AWQ_ERR_ALIGN;
+  if (int e = check_device()) return e;
+  const char* xb = static_cast<const char*>(x);
+  return counted(b200awq::launch_silu_mul(xb, xb + (size_t)d * 2, y, (size_t)m, (size_t)d, (size_t)2 * d, dtype, pdl_enabled(),
+                                          static_cast<cudaStream_t>(stream)),
+                 m);
+}
+
 int gemv_forward_4bit(const void* x, const void* qweight, const void* scales, const void* szeros, void* y, int m, int n,
                       int k, int group_size, int dtype, void* stream) {
   return b200awq_w4a16_gemv(x, qweight, scales, szeros, y, m, n, k, group_size, dtype, stream);
@@ -328,10 +389,11 @@ unsigned long long b200awq_launch_count(void) { return g_launches.load(std::memo
 const char* b200awq_strerror(int code) {
   switch (code) {
     case B200AWQ_OK: return "ok";
-    case B200AWQ_ERR_SHAPE: return "unsupported shape (need n % 8 == 0 [gemm: n % 128 == 0], k % 128 == 0, m >= 1)";
+    case B200AWQ_ERR_SHAPE:
+      return "unsupported shape (need n % 8 == 0 [gemm: n % 128 == 0], k % 128 == 0 [w8a8 gemm: k % 16 == 0], m >= 1)";
     case B200AWQ_ERR_GROUP: return "unsupported group size (only 128)";
     case B200AWQ_ERR_ALIGN: return "null or misaligned pointer (16-byte alignment required)";
-    case B200AWQ_ERR_DTYPE: return "unsupported dtype (fp16 / bf16 only)";
+    case B200AWQ_ERR_DTYPE: return "unsupported dtype (fp16 / bf16 only; gelu_quant: fp16 only)";
     case B200AWQ_ERR_BATCH: return "unsupported batch size for gemv kernel (1..7)";
     case B200AWQ_ERR_WORKSPACE: return "workspace too small";
     case B200AWQ_ERR_DRIVER: return "cuTensorMapEncodeTiled unavailable or failed";

@@ -9,6 +9,7 @@
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
 
+#include <initializer_list>
 #include <map>
 #include <stdexcept>
 
@@ -239,8 +240,148 @@ void rotary_embedding_neox(at::Tensor& positions, at::Tensor& query, at::Tensor&
         false);
 }
 
+// ---------------------------------------------------------------- W8A8 (w8a8/*.cu of the reference)
+// Same argument order, return values and keyword names as the reference (csrc/pybind.cpp:30-37).  Unlike the
+// reference, shapes, dtypes and contiguity are checked, and the launches go to the current stream of the input's
+// device under a device guard.  fp32 activations are not dispatched.
+namespace {
+
+void check_cuda_contig(std::initializer_list<const torch::Tensor*> ts, const char* fn) {
+  for (const torch::Tensor* t : ts) {
+    TORCH_CHECK(t->is_cuda(), fn, ": all tensors must be CUDA tensors");
+    TORCH_CHECK(t->is_contiguous(), fn, ": all tensors must be contiguous");
+  }
+}
+void check_dtype(const torch::Tensor& t, at::ScalarType want, const char* fn, const char* what) {
+  TORCH_CHECK(t.scalar_type() == want, fn, ": ", what, " must be ", want, ", got ", t.scalar_type());
+}
+
+void w8a8_gemm(const torch::Tensor& in, const torch::Tensor& kernel, const torch::Tensor& wscales, const torch::Tensor& ascales,
+               torch::Tensor& out, const torch::Tensor* bias, const char* fn) {
+  std::initializer_list<const torch::Tensor*> all = {&in, &kernel, &wscales, &ascales, &out};
+  check_cuda_contig(all, fn);
+  if (bias) check_cuda_contig({bias}, fn);
+  check_dtype(in, at::ScalarType::Char, fn, "in_feats");
+  check_dtype(kernel, at::ScalarType::Char, fn, "kernel");
+  check_dtype(wscales, at::ScalarType::Half, fn, "wscales");
+  check_dtype(ascales, at::ScalarType::Half, fn, "ascales");
+  check_dtype(out, at::ScalarType::Half, fn, "out_feats");
+  if (bias) check_dtype(*bias, at::ScalarType::Half, fn, "bias");
+  TORCH_CHECK(in.dim() == 2 && kernel.dim() == 2 && out.dim() >= 2, fn, ": in_feats / kernel must be 2-D, out_feats >= 2-D");
+  // reference: M, N from out_feats, K from in_feats (w8a8_gemm_cuda.cu:907-927)
+  const int64_t m = out.size(-2), n = out.size(-1), k = in.size(1);
+  TORCH_CHECK(out.numel() == m * n, fn, ": out_feats must be [M, N]");
+  TORCH_CHECK(in.size(0) == m, fn, ": in_feats has ", in.size(0), " rows, out_feats ", m);
+  TORCH_CHECK(kernel.size(0) == n && kernel.size(1) == k, fn, ": kernel must be [N, K] = [", n, ", ", k, "]");
+  TORCH_CHECK(wscales.numel() >= n && ascales.numel() >= m, fn, ": wscales needs N, ascales M elements");
+  if (bias) TORCH_CHECK(bias->numel() >= n, fn, ": bias needs N elements");
+  if (m == 0 || n == 0) return;
+  const c10::cuda::CUDAGuard guard(in.device());
+  raise(b200awq_w8a8_gemm(in.data_ptr(), kernel.data_ptr(), wscales.data_ptr(), ascales.data_ptr(), bias ? bias->data_ptr() : nullptr,
+                          out.data_ptr(), (int)m, (int)n, (int)k, at::cuda::getCurrentCUDAStream().stream()),
+        false);
+}
+
+int act_dtype(const torch::Tensor& t, const char* fn) {
+  TORCH_CHECK(t.scalar_type() != at::ScalarType::Float, fn, ": fp32 activations are not supported by this build");
+  return dtype_code(t, fn);
+}
+
+}  // namespace
+
+// reference: w8a8/w8a8_gemm_cuda.cu:907-953
+void w8a8_gemm_forward_cuda(torch::Tensor _in_feats, torch::Tensor _kernel, torch::Tensor _wscales, torch::Tensor _ascales,
+                            torch::Tensor _out_feats) {
+  w8a8_gemm(_in_feats, _kernel, _wscales, _ascales, _out_feats, nullptr, "w8a8_gemm_forward_cuda");
+}
+
+// reference: w8a8/w8a8_gemm_cuda.cu:586-633
+void w8a8_gemm_fuse_bias_forward_cuda(torch::Tensor _in_feats, torch::Tensor _kernel, torch::Tensor _wscales,
+                                      torch::Tensor _ascales, torch::Tensor _out_feats, torch::Tensor _bias) {
+  w8a8_gemm(_in_feats, _kernel, _wscales, _ascales, _out_feats, &_bias, "w8a8_gemm_fuse_bias_forward_cuda");
+}
+
+// reference: w8a8/quantization.cu:97-112 (out int8 like input, scale fp16 [tokens])
+void invoke_quant(torch::Tensor& out, torch::Tensor& input, torch::Tensor& scale) {
+  const char* fn = "invoke_quant";
+  check_cuda_contig({&out, &input, &scale}, fn);
+  const int dt = act_dtype(input, fn);
+  check_dtype(out, at::ScalarType::Char, fn, "out");
+  check_dtype(scale, at::ScalarType::Half, fn, "scale");
+  TORCH_CHECK(input.dim() >= 1 && input.size(-1) > 0, fn, ": input must have a last dimension");
+  const int64_t n = input.size(-1), m = input.numel() / n;
+  TORCH_CHECK(out.numel() == input.numel() && scale.numel() >= m, fn, ": out must match input, scale needs one per token");
+  const c10::cuda::CUDAGuard guard(input.device());
+  raise(b200awq_quant_per_token(input.data_ptr(), out.data_ptr(), scale.data_ptr(), (int)m, (int)n, dt,
+                                at::cuda::getCurrentCUDAStream().stream()),
+        false);
+}
+
+// reference: w8a8/layernorm.cu:193-231
+void rms_norm_general(torch::Tensor& out, torch::Tensor& input, torch::Tensor& weight, torch::Tensor& bias, torch::Tensor& scaling,
+                      float epsilon, bool use_per_token_quant) {
+  const char* fn = "rms_norm_general";
+  check_cuda_contig({&out, &input, &weight, &scaling}, fn);
+  const int dt = act_dtype(input, fn);
+  check_dtype(out, at::ScalarType::Char, fn, "out");
+  check_dtype(scaling, at::ScalarType::Half, fn, "scaling");
+  check_dtype(weight, input.scalar_type(), fn, "weight");
+  TORCH_CHECK(input.dim() >= 1 && input.size(-1) > 0, fn, ": input must have a last dimension");
+  const int64_t n = input.size(-1), m = input.numel() / n;
+  TORCH_CHECK(out.numel() == input.numel() && weight.numel() == n, fn, ": out must match input, weight must be [hidden]");
+  const void* beta = nullptr;
+  if (use_per_token_quant) {  // the per-tensor branch of the reference ignores bias
+    check_cuda_contig({&bias}, fn);
+    check_dtype(bias, input.scalar_type(), fn, "bias");
+    TORCH_CHECK(bias.numel() == n, fn, ": bias must be [hidden]");
+    beta = bias.data_ptr();
+    TORCH_CHECK(scaling.numel() >= m, fn, ": scaling needs one element per token");
+  } else {
+    TORCH_CHECK(scaling.numel() >= 1, fn, ": scaling needs one element");
+  }
+  const c10::cuda::CUDAGuard guard(input.device());
+  raise(b200awq_layernorm_quant(input.data_ptr(), weight.data_ptr(), beta, out.data_ptr(), scaling.data_ptr(), (int)m, (int)n,
+                                epsilon, use_per_token_quant ? 1 : 0, dt, at::cuda::getCurrentCUDAStream().stream()),
+        false);
+}
+
+// reference: w8a8/act.cu:120-141 (input [..., 2d] -> new tensor [..., d])
+torch::Tensor silu_and_mul(torch::Tensor& input) {
+  const char* fn = "silu_and_mul";
+  check_cuda_contig({&input}, fn);
+  const int dt = act_dtype(input, fn);
+  TORCH_CHECK(input.dim() >= 1 && input.size(-1) % 2 == 0, fn, ": last dimension must be even");
+  const int64_t d = input.size(-1) / 2, m = d ? input.numel() / (2 * d) : 0;
+  std::vector<int64_t> shape = input.sizes().vec();
+  shape.back() = d;
+  torch::Tensor out = torch::empty(shape, input.options());
+  if (m == 0 || d == 0) return out;
+  const c10::cuda::CUDAGuard guard(input.device());
+  raise(b200awq_silu_and_mul(input.data_ptr(), out.data_ptr(), (int)m, (int)d, dt, at::cuda::getCurrentCUDAStream().stream()),
+        false);
+  return out;
+}
+
+// reference: w8a8/act.cu:82-95 (fp16 only)
+void gelu_and_quant(torch::Tensor& out, torch::Tensor& input, torch::Tensor& scale_out, torch::Tensor& tmp) {
+  const char* fn = "gelu_and_quant";
+  check_cuda_contig({&out, &input, &scale_out, &tmp}, fn);
+  check_dtype(input, at::ScalarType::Half, fn, "input");
+  check_dtype(tmp, at::ScalarType::Half, fn, "tmp");
+  check_dtype(scale_out, at::ScalarType::Half, fn, "scale_out");
+  check_dtype(out, at::ScalarType::Char, fn, "out");
+  TORCH_CHECK(input.dim() >= 1 && input.size(-1) > 0, fn, ": input must have a last dimension");
+  const int64_t n = input.size(-1), m = input.numel() / n;
+  TORCH_CHECK(out.numel() == input.numel() && tmp.numel() >= input.numel() && scale_out.numel() >= m, fn,
+              ": out / tmp must match input, scale_out needs one per token");
+  const c10::cuda::CUDAGuard guard(input.device());
+  raise(b200awq_gelu_quant(input.data_ptr(), out.data_ptr(), scale_out.data_ptr(), tmp.data_ptr(), (int)m, (int)n,
+                           at::cuda::getCurrentCUDAStream().stream()),
+        false);
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "H100 (sm_90a) drop-in for llm-awq's awq_inference_engine (W4A16 path only)";
+  m.doc() = "H100 (sm_90a) drop-in for llm-awq's awq_inference_engine (W4A16 and W8A8 paths)";
   m.def("gemm_forward_cuda_new", &gemm_forward_cuda_new, "New quantized GEMM kernel.");
   m.def("gemv_forward_cuda_new", &gemv_forward_cuda_new, "New quantized GEMV kernel.");
   m.def("layernorm_forward_cuda", &layernorm_forward_cuda, "FasterTransformer layernorm kernel");
@@ -252,6 +393,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         "Fused rope forward function with B,S,D embedding");
   m.def("rotary_embedding_neox", &rotary_embedding_neox, "Apply GPT-NeoX style rotary embedding to query and key");
   m.def("mlp_front_forward_cuda", &mlp_front_forward_cuda, "silu(x Wgate^T) * (x Wup^T) for W4A16 weights, one call");
+  m.def("w8a8_gemm_forward_cuda", &w8a8_gemm_forward_cuda, "our w8a8 gemm kernel");
+  m.def("w8a8_gemm_fuse_bias_forward_cuda", &w8a8_gemm_fuse_bias_forward_cuda, "our w8a8 gemm fused bias kernel");
+  m.def("invoke_quant", &invoke_quant, "fp16->int8 quantization");
+  m.def("rms_norm_general", &rms_norm_general, py::arg("out"), py::arg("input"), py::arg("weight"), py::arg("bias"),
+        py::arg("scaling"), py::arg("epsilon"), py::arg("use_per_token_quant") = true,
+        "LayerNorm + int8 quantization (per token or per tensor)");
+  m.def("silu_and_mul", &silu_and_mul, "Activation function.");
+  m.def("gelu_and_quant", &gelu_and_quant, "Apply gelu act and quant output");
   m.def("set_pdl", [](bool on) { return b200awq_set_pdl(on ? 1 : 0) != 0; }, "programmatic dependent launch on/off");
   m.def("launch_count", []() { return b200awq_launch_count(); }, "kernels launched by libb200awq so far");
   m.def("version", []() { return std::string(b200awq_version()); });

@@ -85,8 +85,10 @@ int launch_decode_mlp_front(const void* x, const void* gqw, const void* gsc, con
                             const void* usz, void* y, int N, int K, int dtype, bool pdl, const DecodeTuning& tune,
                             cudaStream_t stream);
 
-// out = silu(gate) * up over `count` elements, the reference's roundings (silu_mul.cu)
-int launch_silu_mul(const void* gate, const void* up, void* out, size_t count, int dtype, bool pdl, cudaStream_t stream);
+// out = silu(gate) * up over rows x cols elements, the reference's roundings; gate / up rows are in_pitch elements
+// apart, out is dense (silu_mul.cu)
+int launch_silu_mul(const void* gate, const void* up, void* out, size_t rows, size_t cols, size_t in_pitch, int dtype, bool pdl,
+                    cudaStream_t stream);
 
 // single-query (decode-step) attention over tinychat's KV-cache layout + RoPE over [s, b, h, d] (attention.cu)
 size_t attention_workspace_bytes(int batch, int heads, int kv_heads, int head_dim, int max_len);
@@ -107,5 +109,17 @@ int launch_flat(const void* x, const void* qw, const void* sc, const void* sz, v
 
 // RMSNorm over the last dimension, one CTA per row (rmsnorm.cu)
 int launch_rmsnorm(const void* x, const void* gamma, void* y, float eps, int m, int n, int dtype, bool pdl, cudaStream_t stream);
+
+// W8A8 GEMM, int8 x [M, K] and w [N, K], fp16 y [M, N] with the reference's epilogue; bias may be null
+// (w8a8_wgmma.cu).  M >= 1, N % 8 == 0, K % 16 == 0.
+int launch_w8a8_gemm(const void* x, const void* w, const void* wscales, const void* ascales, const void* bias, void* y,
+                     int M, int N, int K, bool pdl, cudaStream_t stream);
+
+// W8A8 row kernels, one CTA per row, rows of at most w8a8_row_limit() elements (w8a8_rowops.cu)
+int w8a8_row_limit();
+int launch_quant_per_token(const void* x, void* q, void* scales, int m, int n, int dtype, bool pdl, cudaStream_t st);
+int launch_layernorm_quant(const void* x, const void* gamma, const void* beta, void* q, void* scale, int m, int n, float eps,
+                           bool per_token, int dtype, bool pdl, cudaStream_t st);
+int launch_gelu_quant(const void* x, void* q, void* scales, void* tmp, int m, int n, bool pdl, cudaStream_t st);
 
 }  // namespace b200awq

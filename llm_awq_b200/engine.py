@@ -49,6 +49,16 @@ def lib() -> ctypes.CDLL:
         L.b200awq_rotary_embedding_neox.restype = ci
         L.b200awq_rmsnorm.argtypes = [vp, vp, vp, ci, ci, ctypes.c_float, ci, vp]
         L.b200awq_rmsnorm.restype = ci
+        L.b200awq_w8a8_gemm.argtypes = [vp, vp, vp, vp, vp, vp, ci, ci, ci, vp]
+        L.b200awq_w8a8_gemm.restype = ci
+        L.b200awq_quant_per_token.argtypes = [vp, vp, vp, ci, ci, ci, vp]
+        L.b200awq_quant_per_token.restype = ci
+        L.b200awq_layernorm_quant.argtypes = [vp, vp, vp, vp, vp, ci, ci, ctypes.c_float, ci, ci, vp]
+        L.b200awq_layernorm_quant.restype = ci
+        L.b200awq_gelu_quant.argtypes = [vp, vp, vp, vp, ci, ci, vp]
+        L.b200awq_gelu_quant.restype = ci
+        L.b200awq_silu_and_mul.argtypes = [vp, vp, ci, ci, ci, vp]
+        L.b200awq_silu_and_mul.restype = ci
         L.b200awq_set_pdl.argtypes = [ci]
         L.b200awq_set_pdl.restype = ci
         L.b200awq_launch_count.restype = ctypes.c_ulonglong
