@@ -11,7 +11,8 @@
 // HBM-bound: algorithmic bytes = 2 * m * n * sizeof(T) (+ n * sizeof(T) of gamma, L2-resident).  One CTA per row;
 // the row is read ONCE with 16-byte loads and kept in registers between the reduction and the scaling (the
 // reference reads it twice with 2-byte loads); all loads of a thread are issued before the first use.  Rows wider
-// than the register budget, or not a multiple of 8 elements, take the generic two-pass kernel.
+// than the register budget, not a multiple of 8 elements, or on pointers that are not 16-byte aligned take the generic
+// two-pass kernel, which sums in the same order.
 #include "w4_common.cuh"
 #include "w4a16_kernels.h"
 
@@ -102,7 +103,9 @@ __global__ void __launch_bounds__(kNormThreads) rmsnorm_rows_kernel(const T* __r
   }
 }
 
-// any n: two passes over the row (the second one hits L1 / L2)
+// any n and alignment: two passes over the row (the second one hits L1 / L2).  The sum of squares runs in the order of
+// rmsnorm_rows_kernel -- thread t owns the 8-element chunks t, t + 256, ..., each in element order -- so a row that
+// either kernel can take gives the same bits on both, whatever the alignment of its pointers.
 template <typename T>
 __global__ void __launch_bounds__(kNormThreads) rmsnorm_generic_kernel(const T* __restrict__ x, const T* __restrict__ gamma,
                                                                        T* __restrict__ y, float eps, int n) {
@@ -111,9 +114,12 @@ __global__ void __launch_bounds__(kNormThreads) rmsnorm_generic_kernel(const T* 
   pdl_wait_prior_grid();
   const T* xr = x + (size_t)blockIdx.x * n;
   float s = 0.f;
-  for (int i = threadIdx.x; i < n; i += kNormThreads) {
-    const float f = elem_to_float<T>(xr[i]);
-    s = fmaf(f, f, s);
+  for (int c = threadIdx.x; c < (n + 7) / 8; c += kNormThreads) {
+    const int end = min(8 * c + 8, n);
+    for (int i = 8 * c; i < end; ++i) {
+      const float f = elem_to_float<T>(xr[i]);
+      s = fmaf(f, f, s);
+    }
   }
   const float r = rsqrtf(block_sum(s, red) / (float)n + eps);
   T* yr = y + (size_t)blockIdx.x * n;
