@@ -51,7 +51,7 @@ extern "C" {
 #define B200AWQ_ERR_BATCH (-5)     /* gemv with m outside 1..7 (reference: gemv_cuda.cu:291-330) */
 #define B200AWQ_ERR_WORKSPACE (-6) /* workspace smaller than b200awq_w4a16_gemm_workspace_bytes */
 #define B200AWQ_ERR_DRIVER (-7)    /* CUDA driver entry point for TMA descriptors unavailable */
-#define B200AWQ_ERR_DEVICE (-8)    /* current device is not compute capability 10.x */
+#define B200AWQ_ERR_DEVICE (-8)    /* current device is not compute capability 9.x */
 #define B200AWQ_ERR_PEERS (-9)     /* bad peer description (world, rank, capacities, null buffers) */
 
 /* Decode path: 1 <= m <= 7 (the reference's GEMV envelope).  n % 8 == 0, k % 128 == 0,
@@ -220,12 +220,15 @@ int gemm_forward_4bit(const void* x, const void* qweight, const void* scales, co
 
 /* Programmatic dependent launch between consecutive launches of this library on one
  * stream (weights of launch i+1 are prefetched while launch i drains).  Default on;
- * B200AWQ_PDL=0 in the environment or b200awq_set_pdl(0) turns it off.  Returns the
- * previous setting. */
+ * b200awq_set_pdl(0) turns it off.  Returns the previous setting. */
 int b200awq_set_pdl(int enable);
 
-/* The library reads its B200AWQ_* environment knobs once, at the first launch.  Tuning / benchmarking tools that
- * change the environment inside one process call this to have them read again (thread-safe). */
+/* Test-only override of the one-token decode kernel's plan, for tests that must run that kernel with a k split or a
+ * ring depth the shape alone would not pick:
+ *   B200AWQ_DECODE_SPLIT  CTAs per cluster = k split (1 to 8) instead of the choice from the shape
+ *   B200AWQ_DECODE_SLOTS  cap on the ring slots; below 3 the kernel declines and the next kernel takes the call
+ * Unset or 0 means "pick from the shape".  Every other kernel configuration is fixed in code.  The library reads the
+ * two variables once, at the first one-token launch; this reads them again (thread-safe). */
 void b200awq_reload_config(void);
 
 /* Number of kernels this library has launched since load (monotonic, per process). */

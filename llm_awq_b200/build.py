@@ -47,14 +47,6 @@ def build_lib(force=False):
     return LIB
 
 
-def build_trace_lib():
-    """Debug variant with per-launch timestamps (-DB200AWQ_TRACE); not part of the product."""
-    out = os.path.join(HERE, "lib", "libb200awq_trace.so")
-    srcs = [os.path.join(CSRC, f) for f in KERNEL_SRCS]
-    _run([os.environ.get("NVCC", "nvcc")] + NVCC_FLAGS + ["-DB200AWQ_TRACE", "-rdc=true", "-shared", "-o", out] + srcs)
-    return out
-
-
 def build_ext(force=False):
     src = os.path.join(CSRC, "torch_ext.cpp")
     if not force and _newer(EXT, [src, LIB, os.path.join(INCLUDE, "b200awq.h"), __file__]):
@@ -79,5 +71,3 @@ def build_all(force=False):
 
 if __name__ == "__main__":
     print(*build_all("--force" in sys.argv), sep="\n")
-    if "--trace" in sys.argv:
-        print(build_trace_lib())

@@ -1,6 +1,6 @@
 // C ABI of libb200awq.so (declared in include/b200awq.h): argument validation, dispatch
-// between the HBM-bound streaming kernel and the wgmma tensor-core kernel, process-wide
-// switches.  No torch types, no allocation, no synchronisation.
+// between the HBM-bound streaming kernels and the wgmma tensor-core kernel, the PDL switch.
+// No torch types, no allocation, no synchronisation.
 #include <atomic>
 #include <cstdint>
 #include <cstdlib>
@@ -12,84 +12,36 @@ namespace {
 
 std::atomic<unsigned long long> g_launches{0};
 
-int env_int(const char* name, int dflt) {
-  const char* v = std::getenv(name);
-  return v && *v ? std::atoi(v) : dflt;
+// Test-only override of the decode kernel's plan (B200AWQ_DECODE_SPLIT, B200AWQ_DECODE_SLOTS; include/b200awq.h), read
+// once on the first one-token launch and again by b200awq_reload_config().  Double-buffered so that a reload never
+// races a reader: readers take a pointer with acquire, writers publish a fully built copy.
+b200awq::DecodeTuning read_decode_tuning() {
+  auto env_int = [](const char* name) {
+    const char* v = std::getenv(name);
+    return v && *v ? std::atoi(v) : 0;
+  };
+  b200awq::DecodeTuning t;
+  t.split = env_int("B200AWQ_DECODE_SPLIT");
+  t.slots = env_int("B200AWQ_DECODE_SLOTS");
+  return t;
 }
 
-// Every environment knob of the library, read ONCE (first launch, or b200awq_reload_config()): the decode path is a
-// few microseconds per call, a dozen getenv() per launch is not free, and the tunings are plain values handed to the
-// launchers -- no mutable globals on the call path.
-struct Config {
-  bool pdl;
-  bool decode;        // B200AWQ_DECODE=0: never use the one-token decode kernel (fp16; bf16 with B200AWQ_DECODE=2)
-  bool decode_bf16;
-  b200awq::DecodeTuning decode_t;
-  bool ring;          // B200AWQ_RING=0: never use the persistent ring kernel
-  int ring_max_m;     // largest token count served by the ring kernel
-  bool flat;          // B200AWQ_SKINNY=stream: never use the wgmma skinny launch
-  int flat_min_m, flat_min_m_longk, flat_max_m;
-  int stream_max_m;
-  b200awq::RingTuning ring_t;
-  b200awq::StreamTuning stream_t;
-  b200awq::FlatTuning flat_t;
-  b200awq::UmmaTuning umma_t;
-};
+b200awq::DecodeTuning g_decode_store[2];
+std::atomic<const b200awq::DecodeTuning*> g_decode{nullptr};
 
-Config read_config() {
-  Config c;
-  c.pdl = env_int("B200AWQ_PDL", 1) != 0;
-  c.decode = env_int("B200AWQ_DECODE", 1) != 0;
-  c.decode_bf16 = env_int("B200AWQ_DECODE", 1) == 2;
-  c.decode_t.split = env_int("B200AWQ_DECODE_SPLIT", 0);
-  c.decode_t.slots = env_int("B200AWQ_DECODE_SLOTS", 0);
-  c.decode_t.warps = env_int("B200AWQ_DECODE_WARPS", 0);
-  c.ring = env_int("B200AWQ_RING", 1) != 0;
-  c.ring_max_m = env_int("B200AWQ_RING_MAX_M", 4);
-  const char* sk = std::getenv("B200AWQ_SKINNY");
-  c.flat = !(sk && sk[0] == 's');
-  // crossovers: the wgmma skinny launch from 5 tokens (from 3 when k is long enough to need a cluster split), the
-  // wgmma tile launch above 16
-  c.flat_min_m = env_int("B200AWQ_FLAT_MIN_M", 5);
-  c.flat_min_m_longk = env_int("B200AWQ_FLAT_MIN_M", 3);
-  c.flat_max_m = env_int("B200AWQ_FLAT_MAX_M", 16);
-  c.stream_max_m = env_int("B200AWQ_STREAM_MAX_M", 16);
-  c.ring_t.mode = env_int("B200AWQ_RING_MODE", -1);
-  c.ring_t.split = env_int("B200AWQ_RING_SPLIT", 0);
-  c.ring_t.slots = env_int("B200AWQ_RING_SLOTS", 0);
-  c.stream_t.mode = env_int("B200AWQ_STREAM_MODE", -1);
-  c.stream_t.kc = env_int("B200AWQ_STREAM_KC", 0);
-  c.stream_t.rpb = env_int("B200AWQ_STREAM_RPB", 0);
-  c.stream_t.pad = env_int("B200AWQ_STREAM_PAD", 0);
-  c.stream_t.rbs = env_int("B200AWQ_STREAM_RBS", 0);
-  c.stream_t.warps = env_int("B200AWQ_STREAM_WARPS", 0);
-  c.flat_t.kc = env_int("B200AWQ_FLAT_KC", 0);
-  c.umma_t.tn = env_int("B200AWQ_UMMA_TN", 0);
-  c.umma_t.max_ctas = env_int("B200AWQ_UMMA_CTAS", 0);
-  c.umma_t.split = env_int("B200AWQ_UMMA_SPLIT", 0);
-  return c;
-}
-
-// Double-buffered so that a reload never races a reader: readers take a pointer with acquire, writers publish a
-// fully built copy.
-Config g_cfg_store[2];
-std::atomic<const Config*> g_cfg{nullptr};
-std::atomic<int> g_pdl_override{-1};  // b200awq_set_pdl(): -1 = follow the environment
-
-const Config& cfg() {
-  const Config* c = g_cfg.load(std::memory_order_acquire);
-  if (!c) {
-    static const Config first = read_config();  // thread-safe one-time initialisation
-    g_cfg.store(&first, std::memory_order_release);
-    c = &first;
+const b200awq::DecodeTuning& decode_tuning() {
+  const b200awq::DecodeTuning* t = g_decode.load(std::memory_order_acquire);
+  if (!t) {
+    static const b200awq::DecodeTuning first = read_decode_tuning();  // thread-safe one-time initialisation
+    g_decode.store(&first, std::memory_order_release);
+    t = &first;
   }
-  return *c;
+  return *t;
 }
 
-bool pdl_enabled() {
-  const int o = g_pdl_override.load(std::memory_order_relaxed);
-  return o < 0 ? cfg().pdl : o != 0;
-}
+std::atomic<bool> g_pdl{true};  // programmatic dependent launch, b200awq_set_pdl()
+
+bool pdl_enabled() { return g_pdl.load(std::memory_order_relaxed); }
 
 bool aligned16(const void* p) { return p && (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
@@ -116,36 +68,43 @@ int check_common(const void* x, const void* qw, const void* sc, const void* sz, 
   return check_device();
 }
 
+// Routing of small token counts.  The one-token decode kernel takes fp16 only: bf16 stays operand-exact in the ring
+// kernel (dropping the bf16 rounding of q s + z would move results by ~1e-3 against the reference).
+constexpr int kRingMaxM = 4;         // largest token count served by the ring kernel
+constexpr int kFlatMinM = 5;         // the wgmma skinny launch from 5 tokens ...
+constexpr int kFlatMinMLongK = 3;    // ... from 3 when k is long enough to need a cluster split (k > 8192) ...
+constexpr int kFlatMaxM = 16;        // ... up to 16; the wgmma tile launch above
+constexpr int kStreamMaxM = 16;      // largest token count served by the streaming kernel
+
+bool use_decode(int m, int dtype) { return m == 1 && dtype == B200AWQ_DTYPE_F16; }
+
 // which kernel serves small token counts beyond the ring kernel's range
-bool use_flat(const Config& c, int m, int n, int k) {
-  const int min_m = k > 8192 ? c.flat_min_m_longk : c.flat_min_m;
-  return c.flat && n % 128 == 0 && m >= min_m && m <= c.flat_max_m;
+bool use_flat(int m, int n, int k) {
+  const int min_m = k > 8192 ? kFlatMinMLongK : kFlatMinM;
+  return n % 128 == 0 && m >= min_m && m <= kFlatMaxM;
 }
 
 // Small token counts (decode and the bottom of the batch sweep): decode (one token) -> ring -> flat -> stream, each returning
 // B200AWQ_ERR_SHAPE (or, for the cluster kernels, a launch-configuration error) when it cannot take the shape.
-int launch_small(const Config& c, const void* x, const void* qw, const void* sc, const void* sz, void* y, int m, int n,
-                 int k, int dtype, cudaStream_t st) {
+int launch_small(const void* x, const void* qw, const void* sc, const void* sz, void* y, int m, int n, int k, int dtype,
+                 cudaStream_t st) {
   int r = B200AWQ_ERR_SHAPE;
-  // one token: fp16 through the int8-digit decode kernel (bf16 stays operand-exact: dropping the bf16 rounding of
-  // q s + z would move results by ~1e-3 against the reference)
-  if (m == 1 && c.decode && (dtype == B200AWQ_DTYPE_F16 || c.decode_bf16))
-    r = b200awq::launch_decode(x, qw, sc, sz, y, n, k, dtype, pdl_enabled(), c.decode_t, st);
+  if (use_decode(m, dtype)) r = b200awq::launch_decode(x, qw, sc, sz, y, n, k, dtype, pdl_enabled(), decode_tuning(), st);
   if (r > 0) {  // a launch-configuration error (e.g. an unschedulable cluster): the kernels below can take the shape
     (void)cudaGetLastError();
     r = B200AWQ_ERR_SHAPE;
   }
-  if (r != 0 && c.ring && m <= c.ring_max_m) r = b200awq::launch_ring(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), c.ring_t, st);
-  if (r != 0 && use_flat(c, m, n, k)) {
-    r = b200awq::launch_flat(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), c.flat_t, st);
+  if (r != 0 && m <= kRingMaxM) r = b200awq::launch_ring(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st);
+  if (r != 0 && use_flat(m, n, k)) {
+    r = b200awq::launch_flat(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st);
     if (r > 0) {  // e.g. an unschedulable cluster shape: not the caller's problem, the streaming kernel can take it
       (void)cudaGetLastError();
       r = B200AWQ_ERR_SHAPE;
     }
   }
-  if (r != 0 && m <= 16 && m <= c.stream_max_m) {
+  if (r != 0 && m <= kStreamMaxM) {
     if (r > 0) (void)cudaGetLastError();
-    r = b200awq::launch_stream(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), c.stream_t, st);
+    r = b200awq::launch_stream(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st);
   }
   return r;
 }
@@ -158,7 +117,7 @@ int b200awq_w4a16_gemv(const void* x, const void* qweight, const void* scales, c
                        int k, int group_size, int dtype, void* stream) {
   if (int e = check_common(x, qweight, scales, szeros, y, m, n, k, group_size, dtype)) return e;
   if (m > 7) return B200AWQ_ERR_BATCH;  // reference envelope: gemv_cuda.cu:291-330
-  const int r = launch_small(cfg(), x, qweight, scales, szeros, y, m, n, k, dtype, static_cast<cudaStream_t>(stream));
+  const int r = launch_small(x, qweight, scales, szeros, y, m, n, k, dtype, static_cast<cudaStream_t>(stream));
   if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
   return r;
 }
@@ -180,8 +139,8 @@ int b200awq_w4a16_gemv_allreduce(const void* x, const void* qweight, const void*
   pa.world = peers->world;
   pa.tok_cap = peers->cap_words / peers->n_max;
   pa.cap = pa.tok_cap * peers->n_max;
-  int r = b200awq::launch_stream(x, qweight, scales, szeros, y, m, n, k, dtype, pdl_enabled(), cfg().stream_t,
-                                 static_cast<cudaStream_t>(stream), &pa);
+  int r = b200awq::launch_stream(x, qweight, scales, szeros, y, m, n, k, dtype, pdl_enabled(), static_cast<cudaStream_t>(stream),
+                                 &pa);
   if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
   return r;
 }
@@ -194,11 +153,10 @@ int b200awq_w4a16_mlp_front(const void* x, const void* gate_qweight, const void*
   if (int e = check_common(x, gate_qweight, gate_scales, gate_szeros, y, m, n, k, group_size, dtype)) return e;
   if (!aligned16(up_qweight) || !aligned16(up_scales) || !aligned16(up_szeros)) return B200AWQ_ERR_ALIGN;
   if (m >= 8 && n % 128) return B200AWQ_ERR_SHAPE;
-  const Config& c = cfg();
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (m == 1 && c.decode && (dtype == B200AWQ_DTYPE_F16 || c.decode_bf16)) {
+  if (use_decode(m, dtype)) {
     const int r = b200awq::launch_decode_mlp_front(x, gate_qweight, gate_scales, gate_szeros, up_qweight, up_scales, up_szeros, y,
-                                                   n, k, dtype, pdl_enabled(), c.decode_t, st);
+                                                   n, k, dtype, pdl_enabled(), decode_tuning(), st);
     if (r == 0) {
       g_launches.fetch_add(1, std::memory_order_relaxed);
       return 0;
@@ -214,9 +172,8 @@ int b200awq_w4a16_mlp_front(const void* x, const void* gate_qweight, const void*
     const void* sc = t ? up_scales : gate_scales;
     const void* sz = t ? up_szeros : gate_szeros;
     int r = B200AWQ_ERR_SHAPE;
-    if (m <= 16) r = launch_small(c, x, qw, sc, sz, t ? u : g, m, n, k, dtype, st);
-    if (r == B200AWQ_ERR_SHAPE && n % 128 == 0)
-      r = b200awq::launch_umma(x, qw, sc, sz, t ? u : g, m, n, k, dtype, pdl_enabled(), c.umma_t, st);
+    if (m <= 16) r = launch_small(x, qw, sc, sz, t ? u : g, m, n, k, dtype, st);
+    if (r == B200AWQ_ERR_SHAPE && n % 128 == 0) r = b200awq::launch_umma(x, qw, sc, sz, t ? u : g, m, n, k, dtype, pdl_enabled(), st);
     if (r != 0) return r;
     g_launches.fetch_add(1, std::memory_order_relaxed);
   }
@@ -289,15 +246,13 @@ int b200awq_w4a16_gemm(const void* x, const void* qweight, const void* scales, c
   (void)workspace_bytes;
   if (int e = check_common(x, qweight, scales, szeros, y, m, n, k, group_size, dtype)) return e;
   if (n % 128) return B200AWQ_ERR_SHAPE;  // reference: N / CTA_N with CTA_N = 128, gemm_cuda.cu:38,1225
-  const Config& c = cfg();
   int r = B200AWQ_ERR_SHAPE;
   // 9..16 tokens on the large layers (>= 48 M weights): the persistent tile launch (split-k); everything else below
   // 17 tokens: the small-token kernels
   const bool big_mid = m > 8 && (long long)n * k >= 48ll * 1000 * 1000;
-  if (m <= 16 && !big_mid) r = launch_small(c, x, qweight, scales, szeros, y, m, n, k, dtype, static_cast<cudaStream_t>(stream));
+  if (m <= 16 && !big_mid) r = launch_small(x, qweight, scales, szeros, y, m, n, k, dtype, static_cast<cudaStream_t>(stream));
   if (r == B200AWQ_ERR_SHAPE)  // 128-channel wgmma tiles; split-k over a cluster for small token counts
-    r = b200awq::launch_umma(x, qweight, scales, szeros, y, m, n, k, dtype, pdl_enabled(), c.umma_t,
-                             static_cast<cudaStream_t>(stream));
+    r = b200awq::launch_umma(x, qweight, scales, szeros, y, m, n, k, dtype, pdl_enabled(), static_cast<cudaStream_t>(stream));
   if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
   return r;
 }
@@ -371,17 +326,13 @@ int gemm_forward_4bit(const void* x, const void* qweight, const void* scales, co
   return b200awq_w4a16_gemm(x, qweight, scales, szeros, y, m, n, k, group_size, dtype, workspace, workspace_bytes, stream);
 }
 
-int b200awq_set_pdl(int enable) {
-  const int prev = pdl_enabled() ? 1 : 0;
-  g_pdl_override.store(enable ? 1 : 0, std::memory_order_relaxed);
-  return prev;
-}
+int b200awq_set_pdl(int enable) { return g_pdl.exchange(enable != 0, std::memory_order_relaxed) ? 1 : 0; }
 
 void b200awq_reload_config(void) {
   static std::atomic<int> which{0};
   const int w = which.fetch_add(1, std::memory_order_relaxed) & 1;
-  g_cfg_store[w] = read_config();
-  g_cfg.store(&g_cfg_store[w], std::memory_order_release);
+  g_decode_store[w] = read_decode_tuning();
+  g_decode.store(&g_decode_store[w], std::memory_order_release);
 }
 
 unsigned long long b200awq_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }

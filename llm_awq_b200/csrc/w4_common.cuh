@@ -72,24 +72,16 @@ __device__ __forceinline__ void unpack_word(uint32_t w, uint32_t (&out)[4]) {
   }
 }
 
-// Raw biased forms, no arithmetic at all: fp16 -> (1024 + q) for j = 0, 2 (nibble in mantissa
+// Raw biased fp16 forms, no arithmetic at all: (1024 + q) for j = 0, 2 (nibble in mantissa
 // bits 0-3 under exponent 2^10) and (64 + q) for j = 1, 3 (nibble in mantissa bits 4-7 under
-// exponent 2^6, magic 0x5400);  bf16 -> (128 + q) for every j.  Only for fp32-accumulating
-// consumers that remove the bias algebraically (w4a16_stream.cu, MODE 2).
-template <typename T>
+// exponent 2^6, magic 0x5400).  Only for fp32-accumulating consumers that remove the bias
+// algebraically (the fp16 MODE 2 of w4a16_ring.cu and w4a16_stream.cu).
 __device__ __forceinline__ void unpack_word_biased(uint32_t w, uint32_t (&out)[4]) {
-  if constexpr (!TypeTraits<T>::kIsBf16) {
-    const uint32_t t = w >> 8;
-    out[0] = and_or(w, 0x000f000fu, 0x64006400u);
-    out[1] = and_or(w, 0x00f000f0u, 0x54005400u);
-    out[2] = and_or(t, 0x000f000fu, 0x64006400u);
-    out[3] = and_or(t, 0x00f000f0u, 0x54005400u);
-  } else {
-    out[0] = and_or(w, 0x000f000fu, 0x43004300u);
-    out[1] = and_or(w >> 4, 0x000f000fu, 0x43004300u);
-    out[2] = and_or(w >> 8, 0x000f000fu, 0x43004300u);
-    out[3] = and_or(w >> 12, 0x000f000fu, 0x43004300u);
-  }
+  const uint32_t t = w >> 8;
+  out[0] = and_or(w, 0x000f000fu, 0x64006400u);
+  out[1] = and_or(w, 0x00f000f0u, 0x54005400u);
+  out[2] = and_or(t, 0x000f000fu, 0x64006400u);
+  out[3] = and_or(t, 0x00f000f0u, 0x54005400u);
 }
 
 // One packed word -> four pairs w~ = rn_T(q * s + z): exact q, then ONE FMA in T
@@ -109,10 +101,7 @@ __device__ __forceinline__ void dequant_word(uint32_t w, uint32_t s2, uint32_t z
   }
 }
 
-__device__ __forceinline__ float bits16_to_float(uint16_t v, bool bf16) {
-  if (bf16) return __uint_as_float((uint32_t)v << 16);
-  return __half2float(__ushort_as_half(v));
-}
+__device__ __forceinline__ float half_bits_to_float(uint16_t v) { return __half2float(__ushort_as_half(v)); }
 
 template <typename T>
 __device__ __forceinline__ T from_float(float v);

@@ -1,4 +1,5 @@
-// One-token W4A16 decode kernel (GEMV, M = 1): the HBM-bound hot path of BASELINE configs[1].
+// One-token fp16 W4A16 decode kernel (GEMV, M = 1): the HBM-bound hot path of BASELINE configs[1].  bf16 tokens are
+// served by w4a16_ring.cu, which keeps the reference's bf16 operand rounding.
 //
 // Replaces the reference's gemv_kernel (quantization_new/gemv/gemv_cuda.cu:74-229).  Third generation of the decode
 // path:
@@ -8,7 +9,7 @@
 //     70..88 KB of copies are in flight per CTA.
 //   * a launch boundary costs microseconds in which nothing can be computed (the previous layer's tail,
 //     griddepcontrol.wait, the staging of the activations).  Two CTAs of consecutive launches co-reside on
-//     every SM (<= 113 KB and <= 102 registers x 320 threads each), the PRODUCER warp never waits for the activations,
+//     every SM (<= 113 KB and <= 56 registers x 576 threads each), the PRODUCER warp never waits for the activations,
 //     so HBM keeps streaming into the next launch's ring through the bubble; the consumers then have to drain the ring
 //     faster than HBM fills it: int8 tensor-core MACs on the packed bytes AS THEY ARE (no dequantisation).
 //
@@ -24,7 +25,7 @@
 // Arithmetic (exact int32 partial sums, fp32 scale application):
 //   a packed byte b = 16 h + l holds two weights of one channel.  With the activation vector split, per 128-k group,
 //   into three signed 7-bit digits of a block-fixed-point number  x_k = e_g (d0 + d1 / 128 + d2 / 16384)  (e_g a power
-//   of two, |d| <= 64: every fp16 / bf16 activation is represented to 2^-21 of the group's largest magnitude),
+//   of two, |d| <= 64: every fp16 activation is represented to 2^-21 of the group's largest magnitude),
 //       raw  = sum_k b_k LO_k,   high = sum_k (b_k & 0xf0) [LO_k | HI_k]      (u8 x s8 IMMA.16832, one LOP3 per word)
 //       sum_k l_k x_lo + h_k x_hi = raw - high.LO + high.HI / 16
 //   the three digits and their LO / HI variants occupy six of the eight "token" columns of the MMA, which one token
@@ -42,36 +43,8 @@
 
 namespace b200awq {
 
-#ifdef B200AWQ_TRACE
-extern __device__ unsigned long long g_trace_buf[1024 * 2 * 8];  // defined in w4a16_stream.cu (trace build, -rdc)
-extern __device__ long long g_ring_dbg[20 * 4];                    // w4a16_ring.cu
-extern __device__ int g_ring_dbg_flags;
-__device__ __forceinline__ unsigned long long dec_globaltimer_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-#define DEC_STAMP(ev)                                                  \
-  if (lane == 0 && (blockIdx.x == 0 || blockIdx.x == gridDim.x - 1)) \
-  g_trace_buf[(((unsigned)a.seq & 1023u) * 2 + (blockIdx.x != 0)) * 8 + (ev)] = dec_globaltimer_ns()
-#define DEC_CLK(var) const long long var = clock64()
-#define DEC_ACC(slot, expr) dbg_acc[slot] += (expr)
-#define DEC_DBG_DECL long long dbg_acc[4] = {0, 0, 0, 0}; const int dbg_flags = g_ring_dbg_flags
-#define DEC_DBG_FLUSH(w)            \
-  if (lane == 0 && blockIdx.x == 0) \
-    for (int i_ = 0; i_ < 4; ++i_) g_ring_dbg[(w) * 4 + i_] = dbg_acc[i_]
-#define DEC_DRY (dbg_flags & 1)
-#else
-#define DEC_STAMP(ev)
-#define DEC_CLK(var)
-#define DEC_ACC(slot, expr)
-#define DEC_DBG_DECL
-#define DEC_DBG_FLUSH(w)
-#define DEC_DRY 0
-#endif
-
-// consumer warps per CTA: 16 (default, <= 56 registers) or 8 (<= 102 registers); warp w owns the groups g % CONS == w of every
-// piece.  + producer warp + finisher warp.
+// 16 consumer warps per CTA; warp w owns the groups g % 16 == w of every piece.  + producer warp + finisher warp.
+constexpr int kDecCons = 16;
 constexpr int kDecPiece = 32;                          // groups of 128 input channels per bulk copy (8 KB of one quad row)
 constexpr int kDecQuadBytes = kDecPiece * 256;         // 4 channels x 4096 k, packed
 constexpr int kDecQuadB = kDecQuadBytes + 16;          // offset of a slot's second quad row (bank skew)
@@ -101,7 +74,6 @@ struct DecArgs {
   int units;    // clusters
   int NS;       // ring slots
   int nrb_max;  // most row blocks any CTA owns
-  int seq;
   DecLayout L;
 };
 
@@ -149,15 +121,13 @@ __device__ __forceinline__ T silu_mul_rounded(float gate_acc, float up_acc) {
 
 // FUSED = false: y = x W~^T.   FUSED = true: y = silu(x Wgate~^T) * (x Wup~^T), both weight sets walked row block by row
 // block through the same ring (SURVEY.md §8f-1: one read of x, two weight streams, one [1, n] write).
-template <typename T, int CONS, bool FUSED>
-__global__ void __launch_bounds__((CONS + 2) * 32, 2) w4a16_decode_kernel(const __grid_constant__ DecArgs a) {
-  constexpr bool kBf16 = TypeTraits<T>::kIsBf16;
-  constexpr int kDecCons = CONS;
+template <bool FUSED>
+__global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(const __grid_constant__ DecArgs a) {
+  using T = __half;
   constexpr int NT = FUSED ? 2 : 1;   // weight sets
   constexpr int RW = 16 * NT;         // partial sums per row block and warp
   extern __shared__ __align__(128) uint8_t smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  DEC_STAMP(0);
   const DecLayout& L = a.L;
   const int S = a.S, NS = a.NS, N = a.N, K = a.K;
   const int rank = (S > 1) ? (int)cluster_ctarank() : 0;
@@ -215,11 +185,6 @@ __global__ void __launch_bounds__((CONS + 2) * 32, 2) w4a16_decode_kernel(const 
     const uint8_t* szb = reinterpret_cast<const uint8_t*>(a.sz);
     int slot = 0, use = 0;
     bool joined = false;  // the CTA barrier is joined once, after the first lap (or at the end of a short walk)
-    DEC_DBG_DECL;
-#ifdef B200AWQ_TRACE
-    const long long clk_begin = clock64();
-    const unsigned long long ns_begin = dec_globaltimer_ns();
-#endif
     for (int rb = 0; rb < nrb; ++rb) {
       const int qb = q_lo + 4 * rb, nqb = min(4, q_hi - qb);  // quad rows of this row block
       for (int pt = 0; pt < npc * NT; ++pt) {
@@ -230,7 +195,6 @@ __global__ void __launch_bounds__((CONS + 2) * 32, 2) w4a16_decode_kernel(const 
         const uint8_t* szt = second ? reinterpret_cast<const uint8_t*>(a.sz2) : szb;
         const int g0 = kg_lo + p * kDecPiece, ng = min(kDecPiece, kg_hi - g0);
         for (int h = 0; h < nqb; h += 2) {  // one slot per octet
-          DEC_CLK(t0);
           if (use > 0) {
             if (!joined) {
               asm volatile("bar.sync 0;" ::: "memory");  // the CTA barrier the other warps wait at (below)
@@ -239,8 +203,6 @@ __global__ void __launch_bounds__((CONS + 2) * 32, 2) w4a16_decode_kernel(const 
             }
             mbar_wait(&empty[slot], (uint32_t)((use - 1) & 1));
           }
-          DEC_CLK(t1);
-          DEC_ACC(0, t1 - t0);
           const int q0 = qb + h, nqs = min(2, nqb - h);
           uint8_t* sw = ring + slot * kDecSlotBytes;
           const uint32_t len = (uint32_t)ng * 256u;
@@ -260,9 +222,6 @@ __global__ void __launch_bounds__((CONS + 2) * 32, 2) w4a16_decode_kernel(const 
             }
           }
           dec_cp_async_arrive(&full[slot]);
-          DEC_CLK(t2);
-          DEC_ACC(1, t2 - t1);
-          DEC_ACC(3, 1);
           if (++slot == NS) slot = 0, ++use;
         }
       }
@@ -272,21 +231,12 @@ __global__ void __launch_bounds__((CONS + 2) * 32, 2) w4a16_decode_kernel(const 
       if (S > 1) dec_cluster_arrive();
     }
     if (S > 1) dec_cluster_wait();
-    DEC_STAMP(1);
-    DEC_DBG_FLUSH(18);  // the probe prints slot 18 as the producer
-#ifdef B200AWQ_TRACE
-    if (lane == 0 && blockIdx.x == 0) {  // SM clock actually delivered over the producer's lifetime: cycles and ns
-      g_ring_dbg[19 * 4 + 0] = clock64() - clk_begin;
-      g_ring_dbg[19 * 4 + 1] = (long long)(dec_globaltimer_ns() - ns_begin);
-    }
-#endif
     return;
   }
 
   asm volatile("bar.sync 0;" ::: "memory");  // barrier inits of both initialising warps are visible (the producer joins after its first lap)
   if (S > 1) dec_cluster_arrive();  // publishes rank 0's exchange barriers to the peers
   if (S > 1) dec_cluster_wait();
-  DEC_STAMP(2);
   // Consumers: everything the first activation loads need is computed BEFORE the dependency wait, and the loads are the
   // first instructions after it (measured: ~470 cycles passed between the wait returning and the loads issuing when the
   // address arithmetic -- kernel parameters from the constant bank, cold instructions -- came after the wait).
@@ -307,10 +257,6 @@ __global__ void __launch_bounds__((CONS + 2) * 32, 2) w4a16_decode_kernel(const 
       asm volatile("ld.global.u32 %0, [%1 + 32];" : "=r"(xb0[i]) : "l"(xfirst[i]) : "memory");
     }
   }
-#ifdef B200AWQ_TRACE
-  const long long clk_wait = clock64();
-#endif
-  DEC_STAMP(3);
 
   if (warp == kDecCons + 1) {
     // ------------------------------------------------------------------ finisher
@@ -381,7 +327,6 @@ __global__ void __launch_bounds__((CONS + 2) * 32, 2) w4a16_decode_kernel(const 
         finish(r, f0, fch);
       }
     }
-    DEC_STAMP(6);
     return;
   }
 
@@ -404,9 +349,6 @@ __global__ void __launch_bounds__((CONS + 2) * 32, 2) w4a16_decode_kernel(const 
     uint8_t* xd = smem + L.x;
     for (int G0 = warp; G0 < ngr; G0 += kMaxOwn * kDecCons) {
       uint32_t xa[kMaxOwn], xb[kMaxOwn];
-#ifdef B200AWQ_TRACE
-      const long long ld_t0 = clock64();
-#endif
 #pragma unroll
       for (int i = 0; i < kMaxOwn; ++i) {
         if (G0 == warp) {  // the first batch was loaded right behind the dependency wait
@@ -417,15 +359,6 @@ __global__ void __launch_bounds__((CONS + 2) * 32, 2) w4a16_decode_kernel(const 
           xa[i] = src[0], xb[i] = src[8];
         }
       }
-#ifdef B200AWQ_TRACE
-      if (G0 == warp && warp == 0 && blockIdx.x == 0) {  // latency of the first activation loads of warp 0 (cycles)
-        const uint32_t dep = xa[0] ^ xb[0] ^ xa[kMaxOwn - 1] ^ xb[kMaxOwn - 1];
-        long long ld_t1 = dep == 0x9e3779b9u ? 1 : 0;  // a real dependency: the clock below is read after the data arrived
-        asm volatile("" ::"l"(ld_t1) : "memory");
-        ld_t1 += clock64();
-        if (lane == 0) g_ring_dbg[19 * 4 + 2] = ld_t1 - ld_t0, g_ring_dbg[19 * 4 + 3] = ld_t0 - clk_wait;
-      }
-#endif
 #pragma unroll
       for (int i = 0; i < kMaxOwn; ++i) {
         const int Gl = G0 + i * kDecCons;
@@ -433,19 +366,15 @@ __global__ void __launch_bounds__((CONS + 2) * 32, 2) w4a16_decode_kernel(const 
         float f[4];  // byte order of the word: pair A element 0, pair B element 0, pair A element 1, pair B element 1
         {
           float2 pa, pb;
-          if constexpr (kBf16) pa = __bfloat1622float2(u32_as_b2(xa[i])), pb = __bfloat1622float2(u32_as_b2(xb[i]));
-          else pa = __half22float2(u32_as_h2(xa[i])), pb = __half22float2(u32_as_h2(xb[i]));
+          pa = __half22float2(u32_as_h2(xa[i])), pb = __half22float2(u32_as_h2(xb[i]));
           f[0] = pa.x, f[1] = pb.x, f[2] = pa.y, f[3] = pb.y;
         }
         // non-negative floats order like their bit patterns: the group's largest magnitude with one integer REDUX
         const uint32_t am = max(max(__float_as_uint(fabsf(f[0])), __float_as_uint(fabsf(f[1]))),
                                 max(__float_as_uint(fabsf(f[2])), __float_as_uint(fabsf(f[3]))));
         const int ex = (int)(__reduce_max_sync(0xffffffffu, am) >> 23);
-#ifdef B200AWQ_TRACE
-        if (i == 0 && G0 == warp) { DEC_STAMP(7); }  // the activation loads have returned
-#endif
-        // e = 2^(floor(log2 amax) - 5): |x| / e < 64.  Groups whose largest magnitude is below 2^-121 (bf16 only)
-        // count as zero.
+        // e = 2^(floor(log2 amax) - 5): |x| / e < 64.  Groups whose largest magnitude is below 2^-121 (all-zero
+        // groups: every nonzero fp16 value is at least 2^-24) count as zero.
         const bool nz = ex >= 6;
         const float inv_e = nz ? __uint_as_float((uint32_t)(259 - ex) << 23) : 0.f;
         const float e = nz ? __uint_as_float((uint32_t)(ex - 5) << 23) : 0.f;
@@ -482,7 +411,6 @@ __global__ void __launch_bounds__((CONS + 2) * 32, 2) w4a16_decode_kernel(const 
     }
     __syncwarp();
   }
-  DEC_STAMP(4);
 
   // ldmatrix.x4 addresses of this lane: matrix i = lane >> 3 is (octet i & 1, 32-k block i >> 1 [+ 2 for the second
   // instruction]), row = channel lane & 7 of that octet (quad row (lane & 7) >> 2, row (lane & 3) of the 128-byte
@@ -501,7 +429,6 @@ __global__ void __launch_bounds__((CONS + 2) * 32, 2) w4a16_decode_kernel(const 
   const int zero4[4] = {0, 0, 0, 0};
 
   int slot = 0, use = 0;
-  DEC_DBG_DECL;
   for (int rb = 0; rb < nrb; ++rb) {
     const int nqb = min(4, nq - 4 * rb);
     const bool two = nqb > 2;  // second octet present
@@ -512,50 +439,42 @@ __global__ void __launch_bounds__((CONS + 2) * 32, 2) w4a16_decode_kernel(const 
       const int ng = min(kDecPiece, ngr - p * kDecPiece);
       int slotB = slot, useB = use;
       if (two && ++slotB == NS) slotB = 0, ++useB;
-      DEC_CLK(t0);
       mbar_wait(&full[slot], (uint32_t)(use & 1));
       if (two) mbar_wait(&full[slotB], (uint32_t)(useB & 1));
-      DEC_CLK(t1);
-      DEC_ACC(0, t1 - t0);
       const uint32_t sa_u32 = ring_u32 + (uint32_t)slot * kDecSlotBytes;
       const uint32_t sb_u32 = ring_u32 + (uint32_t)slotB * kDecSlotBytes;  // == sa_u32 without a second octet
       const uint32_t w_lane = (ldsm_b ? sb_u32 : sa_u32) + ldsm_off;
-      if (!DEC_DRY) {
-        // per-item bases; a group adds its index times a constant (folded into the instructions for the two groups of
-        // a full piece)
-        const uint32_t xd_item = xd_lane + (uint32_t)(p * kDecPiece) * kDecGroupBytes;
-        const uint32_t gx_item = gx_lane + (uint32_t)(p * kDecPiece) * 16u;
-        const uint32_t cA_item = sa_u32 + sc_off + coef_sel, cB_item = sb_u32 + sc_off + coef_sel;
-        auto mac_group = [&](const uint32_t gi) {
-          uint32_t w0[4], w1[4];
-          dec_ldsm4(w0, w_lane + gi * 256u);
-          dec_ldsm4(w1, w_lane + gi * 256u + 128u);
-          const uint4 bv = dec_lds128(xd_item + gi * (uint32_t)kDecGroupBytes);
-          float gv;
-          asm volatile("ld.shared.f32 %0, [%1];" : "=f"(gv) : "r"(gx_item + gi * 16u));
-          const uint16_t cA = dec_lds16(cA_item + gi * 8u), cB = dec_lds16(cB_item + gi * 8u);
-          int accR[4], accH[4];
-          dec_imma(accR, w0[0], w0[1], w0[2], w0[3], bv.x, bv.y, zero4);
-          dec_imma(accH, w0[0] & 0xf0f0f0f0u, w0[1] & 0xf0f0f0f0u, w0[2] & 0xf0f0f0f0u, w0[3] & 0xf0f0f0f0u, bv.x, bv.y, zero4);
-          dec_imma(accR, w1[0], w1[1], w1[2], w1[3], bv.z, bv.w, accR);
-          dec_imma(accH, w1[0] & 0xf0f0f0f0u, w1[1] & 0xf0f0f0f0u, w1[2] & 0xf0f0f0f0u, w1[3] & 0xf0f0f0f0u, bv.z, bv.w, accH);
-          // digit lanes: columns 2 tig, 2 tig + 1 = digit tig: low-nibble sum accR[0] - accH[0], high-nibble sum accH[1] / 16
-          // -> T16 = 16 (accR[0] - accH[0]) + accH[1] (the 1 / 16 is folded into gv); zero-term lanes: T = 1, gv = X_g
-          const float t0f = tig == 3 ? 1.f : (float)(((accR[0] - accH[0]) << 4) + accH[1]);
-          const float t1f = tig == 3 ? 1.f : (float)(((accR[2] - accH[2]) << 4) + accH[3]);
-          y0 = fmaf(bits16_to_float(cA, kBf16) * gv, t0f, y0);
-          y1 = fmaf(bits16_to_float(cB, kBf16) * gv, t1f, y1);  // second octet absent: a copy of the first, never stored
-        };
-        if (ng == kDecPiece && kDecCons == 16) {
-          mac_group((uint32_t)warp);
-          mac_group((uint32_t)warp + 16u);
-        } else {
-          for (int gi = warp; gi < ng; gi += kDecCons) mac_group((uint32_t)gi);
-        }
+      // per-item bases; a group adds its index times a constant (folded into the instructions for the two groups of
+      // a full piece)
+      const uint32_t xd_item = xd_lane + (uint32_t)(p * kDecPiece) * kDecGroupBytes;
+      const uint32_t gx_item = gx_lane + (uint32_t)(p * kDecPiece) * 16u;
+      const uint32_t cA_item = sa_u32 + sc_off + coef_sel, cB_item = sb_u32 + sc_off + coef_sel;
+      auto mac_group = [&](const uint32_t gi) {
+        uint32_t w0[4], w1[4];
+        dec_ldsm4(w0, w_lane + gi * 256u);
+        dec_ldsm4(w1, w_lane + gi * 256u + 128u);
+        const uint4 bv = dec_lds128(xd_item + gi * (uint32_t)kDecGroupBytes);
+        float gv;
+        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(gv) : "r"(gx_item + gi * 16u));
+        const uint16_t cA = dec_lds16(cA_item + gi * 8u), cB = dec_lds16(cB_item + gi * 8u);
+        int accR[4], accH[4];
+        dec_imma(accR, w0[0], w0[1], w0[2], w0[3], bv.x, bv.y, zero4);
+        dec_imma(accH, w0[0] & 0xf0f0f0f0u, w0[1] & 0xf0f0f0f0u, w0[2] & 0xf0f0f0f0u, w0[3] & 0xf0f0f0f0u, bv.x, bv.y, zero4);
+        dec_imma(accR, w1[0], w1[1], w1[2], w1[3], bv.z, bv.w, accR);
+        dec_imma(accH, w1[0] & 0xf0f0f0f0u, w1[1] & 0xf0f0f0f0u, w1[2] & 0xf0f0f0f0u, w1[3] & 0xf0f0f0f0u, bv.z, bv.w, accH);
+        // digit lanes: columns 2 tig, 2 tig + 1 = digit tig: low-nibble sum accR[0] - accH[0], high-nibble sum accH[1] / 16
+        // -> T16 = 16 (accR[0] - accH[0]) + accH[1] (the 1 / 16 is folded into gv); zero-term lanes: T = 1, gv = X_g
+        const float t0f = tig == 3 ? 1.f : (float)(((accR[0] - accH[0]) << 4) + accH[1]);
+        const float t1f = tig == 3 ? 1.f : (float)(((accR[2] - accH[2]) << 4) + accH[3]);
+        y0 = fmaf(half_bits_to_float(cA) * gv, t0f, y0);
+        y1 = fmaf(half_bits_to_float(cB) * gv, t1f, y1);  // second octet absent: a copy of the first, never stored
+      };
+      if (ng == kDecPiece) {  // a full piece: two groups per warp
+        mac_group((uint32_t)warp);
+        mac_group((uint32_t)warp + 16u);
+      } else {
+        for (int gi = warp; gi < ng; gi += kDecCons) mac_group((uint32_t)gi);
       }
-      DEC_CLK(t2);
-      DEC_ACC(1, t2 - t1);
-      DEC_ACC(3, 1);
       __syncwarp();
       if (lane == 0) {
         mbar_arrive(&empty[slot]);  // the slots' words are in registers / consumed
@@ -565,7 +484,6 @@ __global__ void __launch_bounds__((CONS + 2) * 32, 2) w4a16_decode_kernel(const 
       if (++slot == NS) slot = 0, ++use;
     }
     // digits live in different lanes (tig): add them, then this warp's 16 partial sums -> red[rb % kDecRed][warp]
-    DEC_CLK(t3);
     y0 += __shfl_xor_sync(0xffffffffu, y0, 1);
     y1 += __shfl_xor_sync(0xffffffffu, y1, 1);
     y0 += __shfl_xor_sync(0xffffffffu, y0, 2);
@@ -590,11 +508,7 @@ __global__ void __launch_bounds__((CONS + 2) * 32, 2) w4a16_decode_kernel(const 
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(&rbfull[rs]);
-    DEC_CLK(t4);
-    DEC_ACC(2, t4 - t3);
   }
-  DEC_STAMP(5);
-  DEC_DBG_FLUSH(warp);
 }
 
 // ------------------------------------------------------------------------------------ host
@@ -613,11 +527,6 @@ int dec_sm_count() {
   return cnt[dev];
 }
 
-int next_dec_seq() {
-  static int seq = 0;
-  return seq++;
-}
-
 }  // namespace
 
 namespace {
@@ -625,7 +534,7 @@ int launch_decode_impl(const void* x, const void* qw, const void* sc, const void
                        const void* sz2, void* y, int N, int K, int dtype, bool pdl, const DecodeTuning& tune, cudaStream_t stream) {
   const bool fused = qw2 != nullptr;
   const int nt = fused ? 2 : 1;
-  if (N % 8 || K % kGroup) return B200AWQ_ERR_SHAPE;
+  if (dtype != B200AWQ_DTYPE_F16 || N % 8 || K % kGroup) return B200AWQ_ERR_SHAPE;
   const int nsm = dec_sm_count();
   if (nsm < 1) return B200AWQ_ERR_SHAPE;
   const int G = K / kGroup, Q = N / 4;
@@ -650,7 +559,6 @@ int launch_decode_impl(const void* x, const void* qw, const void* sc, const void
   if (S > 1 && (nsm % S || G < S)) S = 1;
   a.S = S;
   a.units = nsm / S;
-  a.seq = next_dec_seq();
   const int nq_max = (Q + a.units - 1) / a.units;
   const int nrb_max = (nq_max + 3) / 4;
   if (nrb_max > kDecMaxRb || (long long)Q * (a.units + 1) >= (1ll << 31)) return B200AWQ_ERR_SHAPE;
@@ -660,10 +568,9 @@ int launch_decode_impl(const void* x, const void* qw, const void* sc, const void
   int off = 0;
   L.bars = off, off += 8 * (2 * kDecMaxSlots + 2 * kDecRed + kDecMaxRb);
   off = (off + 127) & ~127;
-  const int cons = tune.warps == 8 ? 8 : 16;
   L.x = off, off += ngr * kDecGroupBytes;
   L.gx = off, off += ngr * 4 * 4;
-  L.red = off, off += kDecRed * cons * 16 * nt * 4;
+  L.red = off, off += kDecRed * kDecCons * 16 * nt * 4;
   L.xchg = off, off += S * nrb_max * 16 * nt * 4;  // the peers' sums (S - 1 regions) + rank 0's own parked sums
   off = (off + 127) & ~127;
   L.ring = off;
@@ -674,26 +581,18 @@ int launch_decode_impl(const void* x, const void* qw, const void* sc, const void
   a.NS = ns;
   L.total = off + ns * kDecSlotBytes;
 
-  static bool attr_set[2][2][2][32] = {};
+  static bool attr_set[2][32] = {};
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return B200AWQ_ERR_DEVICE;
-  const int ti = dtype == B200AWQ_DTYPE_F16 ? 0 : 1;
-  const int ci = cons == 8 ? 0 : 1;
-  const int fi = fused ? 1 : 0;
-  const void* kerns[2][2][2] = {
-      {{(const void*)w4a16_decode_kernel<__half, 8, false>, (const void*)w4a16_decode_kernel<__half, 8, true>},
-       {(const void*)w4a16_decode_kernel<__half, 16, false>, (const void*)w4a16_decode_kernel<__half, 16, true>}},
-      {{(const void*)w4a16_decode_kernel<__nv_bfloat16, 8, false>, (const void*)w4a16_decode_kernel<__nv_bfloat16, 8, true>},
-       {(const void*)w4a16_decode_kernel<__nv_bfloat16, 16, false>, (const void*)w4a16_decode_kernel<__nv_bfloat16, 16, true>}}};
-  const void* kern = kerns[ti][ci][fi];
-  if (!attr_set[ti][ci][fi][dev & 31]) {
+  const void* kern = fused ? (const void*)w4a16_decode_kernel<true> : (const void*)w4a16_decode_kernel<false>;
+  if (!attr_set[fused][dev & 31]) {
     if (cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemBudget)) return (int)e;
     cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    attr_set[ti][ci][fi][dev & 31] = true;
+    attr_set[fused][dev & 31] = true;
   }
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3((unsigned)(a.units * a.S));
-  cfg.blockDim = dim3((unsigned)((cons + 2) * 32));
+  cfg.blockDim = dim3((unsigned)((kDecCons + 2) * 32));
   cfg.dynamicSmemBytes = (size_t)L.total;
   cfg.stream = stream;
   cudaLaunchAttribute attrs[2];

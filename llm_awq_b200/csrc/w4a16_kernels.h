@@ -21,20 +21,9 @@ inline cudaError_t ensure_dyn_smem(K kern, int bytes, bool (&flags)[32]) {
   return e;
 }
 
-struct StreamTuning {
-  int mode = -1;  // -1 = auto (fp16: 2, bf16: 0); 0 operand-exact, 2 group-factored    [env B200AWQ_STREAM_MODE]
-  int kc = 0;     // 0 = auto, else input channels per CTA (K / kc in {1,2,4,8})       [env B200AWQ_STREAM_KC]
-  int rpb = 0;    // 0 = auto, else 1024-k rounds per prefetch barrier (copy = 2 rpb KB) [env B200AWQ_STREAM_RPB]
-  int rbs = 0;    // 0 = auto, else row blocks per CTA (1 or 2)                        [env B200AWQ_STREAM_RBS]
-  int warps = 0;  // 0 = auto, else 8 or 16 warps per CTA                              [env B200AWQ_STREAM_WARPS]
-  int pad = 0;    // extra dynamic smem bytes per CTA (co-residency limiter, tuning)     [env B200AWQ_STREAM_PAD]
-};
-
-struct UmmaTuning {
-  int tn = 0;      // 0 = auto, else token tile (16 / 32 / 64 / 128)    [env B200AWQ_UMMA_TN]
-  int max_ctas = 0;  // 0 = one per SM                                   [env B200AWQ_UMMA_CTAS]
-  int split = 0;     // 0 = auto, 1 = never, 2/4/8 = split k over a cluster [env B200AWQ_UMMA_SPLIT]
-};
+// Every launcher below picks its kernel configuration (instantiation, k split, grid, ring depth, shared-memory size)
+// from the shape and the device's SM count alone; the constants behind those choices live in the launchers.  The one
+// exception is DecodeTuning: a test-only override of the decode kernel's plan (include/b200awq.h).
 
 // Row-parallel tensor parallelism: the GEMV epilogue exchanges fp32 partial sums with the peer GPUs through
 // symmetric (peer-mapped) buffers over NVLink and reduces them in the same kernel (w4a16_stream.cu).
@@ -46,37 +35,28 @@ struct PeerArgs {
   int tok_cap;                  // tokens a region is laid out for: word slot = channel * tok_cap + token
 };
 
-struct FlatTuning {
-  int kc = 0;  // 0 = auto, else input channels per CTA (K / kc <= 8)   [env B200AWQ_FLAT_KC]
-};
-
 // HBM-bound streaming kernel, 1 <= M <= 16 (w4a16_stream.cu)
 int launch_stream(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                  bool pdl, const StreamTuning& tune, cudaStream_t stream, const PeerArgs* peers = nullptr);
+                  bool pdl, cudaStream_t stream, const PeerArgs* peers = nullptr);
 
 // TMA + wgmma tensor-core kernel, any M, N % 128 == 0 (w4a16_wgmma.cu)
 int launch_umma(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                bool pdl, const UmmaTuning& tune, cudaStream_t stream);
-
-struct RingTuning {
-  int mode = -1;   // -1 = auto (fp16: 2, bf16: 0); 0 or 2                               [env B200AWQ_RING_MODE]
-  int split = 0;   // 0 = auto, 1 = no k split, 2 = k split over a 2-CTA cluster      [env B200AWQ_RING_SPLIT]
-  int slots = 0;   // 0 = as many ring slots as fit next to a second CTA, else a cap  [env B200AWQ_RING_SLOTS]
-};
+                bool pdl, cudaStream_t stream);
 
 // persistent warp-specialised decode kernel, 1 <= M <= 8 (w4a16_ring.cu); returns B200AWQ_ERR_SHAPE when the
 // activations do not fit next to a useful ring (the caller falls back to the kernels below)
 int launch_ring(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                bool pdl, const RingTuning& tune, cudaStream_t stream);
+                bool pdl, cudaStream_t stream);
 
+// Test-only override of the decode kernel's plan (env B200AWQ_DECODE_SPLIT / B200AWQ_DECODE_SLOTS, api.cu): the
+// default-constructed value means "pick from the shape".
 struct DecodeTuning {
-  int split = 0;   // 0 = auto, else CTAs per cluster = k split (1, 2, 4, 8)            [env B200AWQ_DECODE_SPLIT]
-  int slots = 0;   // 0 = as many ring slots as fit next to a second CTA, else a cap    [env B200AWQ_DECODE_SLOTS]
-  int warps = 0;   // consumer warps per CTA: 8, else 16                                  [env B200AWQ_DECODE_WARPS]
+  int split = 0;   // 0 = auto, else CTAs per cluster = k split (1 to 8)
+  int slots = 0;   // 0 = as many ring slots as fit next to a second CTA, else a cap
 };
 
-// one-token decode kernel: 8 KB bulk copies, int8-digit tensor-core MACs (w4a16_decode.cu); returns
-// B200AWQ_ERR_SHAPE when the activations do not fit next to a useful ring (the caller falls back)
+// one-token fp16 decode kernel: 8 KB bulk copies, int8-digit tensor-core MACs (w4a16_decode.cu); returns
+// B200AWQ_ERR_SHAPE for bf16 and when the activations do not fit next to a useful ring (the caller falls back)
 int launch_decode(const void* x, const void* qw, const void* sc, const void* sz, void* y, int N, int K, int dtype, bool pdl,
                   const DecodeTuning& tune, cudaStream_t stream);
 
@@ -105,7 +85,7 @@ int launch_rope_neox(const long long* positions, void* query, void* key, const v
 
 // the same kernel for skinny batches, 1 <= M <= 64, N % 128 == 0: one CTA per tile and k slice (w4a16_wgmma.cu)
 int launch_flat(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                bool pdl, const FlatTuning& tune, cudaStream_t stream);
+                bool pdl, cudaStream_t stream);
 
 // RMSNorm over the last dimension, one CTA per row (rmsnorm.cu)
 int launch_rmsnorm(const void* x, const void* gamma, void* y, float eps, int m, int n, int dtype, bool pdl, cudaStream_t stream);

@@ -39,35 +39,6 @@
 
 namespace b200awq {
 
-#ifdef B200AWQ_TRACE
-extern __device__ unsigned long long g_trace_buf[1024 * 2 * 8];  // defined in w4a16_stream.cu (trace build, -rdc)
-__device__ __forceinline__ unsigned long long ring_globaltimer_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-#define RING_STAMP(ev)                                                       \
-  if (lane == 0 && (blockIdx.x == 0 || blockIdx.x == gridDim.x - 1))       \
-  g_trace_buf[(((unsigned)a.seq & 1023u) * 2 + (blockIdx.x != 0)) * 8 + (ev)] = ring_globaltimer_ns()
-// per-warp cycle accounting of CTA 0 (last launch wins): [warp 0..10][0..3] = cycles waiting / working / hand-off / count
-__device__ long long g_ring_dbg[20 * 4];
-__device__ int g_ring_dbg_flags;  // bit 0: consumers skip the math (streaming limit of the ring), bit 1: skip x staging
-#define RING_CLK(var) const long long var = clock64()
-#define RING_ACC(slot, expr) dbg_acc[slot] += (expr)
-#define RING_DBG_DECL long long dbg_acc[4] = {0, 0, 0, 0}; const int dbg_flags = g_ring_dbg_flags
-#define RING_DBG_FLUSH(w)                                        \
-  if (lane == 0 && blockIdx.x == 0)                              \
-    for (int i_ = 0; i_ < 4; ++i_) g_ring_dbg[(w) * 4 + i_] = dbg_acc[i_]
-#define RING_DRY (dbg_flags & 1)
-#else
-#define RING_STAMP(ev)
-#define RING_CLK(var)
-#define RING_ACC(slot, expr)
-#define RING_DBG_DECL
-#define RING_DBG_FLUSH(w)
-#define RING_DRY 0
-#endif
-
 constexpr int kRingCons = 8;                          // consumer warps
 constexpr int kRingProd = 2;                          // producer warps (one thread's bulk-copy issue rate is ~45 B/clk)
 constexpr int kRingThreads = (kRingCons + kRingProd + 1) * 32;  // + finisher warp
@@ -94,8 +65,6 @@ struct RingArgs {
   int units;  // clusters
   int NS;     // ring slots
   int Mp;     // power of two >= M
-  int nrb_max;  // most row blocks any CTA owns
-  int seq;
   RingLayout L;
 };
 
@@ -129,10 +98,10 @@ __device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 1, %0;" 
 //   xsrc  this lane's 64 bytes of staged activations (token g, word slot tig) of the group
 //   ssrc  &scales[group][channel g] in the slot (zeros 512 B further, channel 8 + g 16 B further)
 //   csrc  &xsum[token 2 tig][group] (MODE 2)
-template <typename T, int MODE, bool M1, bool TWO>
+template <typename T, bool M1, bool TWO>
 __device__ __forceinline__ void group_step(uint32_t wsrc, uint32_t xsrc, uint32_t ssrc, const float2* csrc, int cstride,
                                            bool live, uint32_t (&xq)[16], float (&yacc)[4], float (&yacc2)[4]) {
-  constexpr bool kBf16 = TypeTraits<T>::kIsBf16;
+  constexpr int MODE = TypeTraits<T>::kIsBf16 ? 0 : 2;
   uint32_t wa[4], wb[4] = {0u, 0u, 0u, 0u};
   ldsm4(wa, wsrc);
   if (TWO) ldsm4(wb, wsrc + 2 * kQS);
@@ -145,7 +114,7 @@ __device__ __forceinline__ void group_step(uint32_t wsrc, uint32_t xsrc, uint32_
   }
   const uint16_t s_a = lds16(ssrc), z_a = lds16(ssrc + 512);
   const uint16_t s_b = TWO ? lds16(ssrc + 16) : (uint16_t)0, z_b = TWO ? lds16(ssrc + 528) : (uint16_t)0;
-  if (MODE == 0) {
+  if constexpr (MODE == 0) {
     const uint32_t sa2 = splat16(s_a), za2 = splat16(z_a), sb2 = splat16(s_b), zb2 = splat16(z_b);
 #pragma unroll
     for (int m = 0; m < 4; ++m) {
@@ -162,18 +131,18 @@ __device__ __forceinline__ void group_step(uint32_t wsrc, uint32_t xsrc, uint32_
 #pragma unroll
     for (int m = 0; m < 4; ++m) {
       uint32_t oa[4], ob[4] = {0u, 0u, 0u, 0u};
-      unpack_word_biased<T>(wa[m], oa);
-      if (TWO) unpack_word_biased<T>(wb[m], ob);
+      unpack_word_biased(wa[m], oa);
+      if (TWO) unpack_word_biased(wb[m], ob);
       mma_16816<T>(part[m], oa[0], ob[0], oa[1], ob[1], xq[4 * m], xq[4 * m + 1], zero4);
       mma_16816<T>(part[m], oa[2], ob[2], oa[3], ob[3], xq[4 * m + 2], xq[4 * m + 3], part[m]);
     }
     // part[.][0..1]: (channel g, tokens 2 tig, + 1); part[.][2..3]: channel 8 + g
-    const float sa = bits16_to_float(s_a, kBf16), za = bits16_to_float(z_a, kBf16);
+    const float sa = half_bits_to_float(s_a), za = half_bits_to_float(z_a);
     const float2 c0 = csrc[0];
     const float p0 = (part[0][0] + part[1][0]) + (part[2][0] + part[3][0]);
     yacc[0] = fmaf(za, c0.x, fmaf(sa, p0 - c0.y, yacc[0]));
     if (TWO) {
-      const float sbf = bits16_to_float(s_b, kBf16), zb = bits16_to_float(z_b, kBf16);
+      const float sbf = half_bits_to_float(s_b), zb = half_bits_to_float(z_b);
       const float p2 = (part[0][2] + part[1][2]) + (part[2][2] + part[3][2]);
       yacc[2] = fmaf(zb, c0.x, fmaf(sbf, p2 - c0.y, yacc[2]));
     }
@@ -182,7 +151,7 @@ __device__ __forceinline__ void group_step(uint32_t wsrc, uint32_t xsrc, uint32_
       const float p1 = (part[0][1] + part[1][1]) + (part[2][1] + part[3][1]);
       yacc[1] = fmaf(za, c1.x, fmaf(sa, p1 - c1.y, yacc[1]));
       if (TWO) {
-        const float sbf = bits16_to_float(s_b, kBf16), zb = bits16_to_float(z_b, kBf16);
+        const float sbf = half_bits_to_float(s_b), zb = half_bits_to_float(z_b);
         const float p3 = (part[0][3] + part[1][3]) + (part[2][3] + part[3][3]);
         yacc[3] = fmaf(zb, c1.x, fmaf(sbf, p3 - c1.y, yacc[3]));
       }
@@ -190,12 +159,11 @@ __device__ __forceinline__ void group_step(uint32_t wsrc, uint32_t xsrc, uint32_
   }
 }
 
-template <typename T, int MODE, bool M1>
+template <typename T, bool M1>
 __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __grid_constant__ RingArgs a) {
-  constexpr bool kBf16 = TypeTraits<T>::kIsBf16;
+  constexpr int MODE = TypeTraits<T>::kIsBf16 ? 0 : 2;  // see the header comment
   extern __shared__ __align__(128) uint8_t smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  RING_STAMP(0);
   const RingLayout& L = a.L;
   const int S = a.S, NS = a.NS, N = a.N, K = a.K, M = a.M;
   const int rank = (S > 1) ? (int)cluster_ctarank() : 0;
@@ -250,15 +218,11 @@ __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __gri
     const uint8_t* szb = reinterpret_cast<const uint8_t*>(a.sz);
     int slot = 0, use = 0, rb = 0, j = 0;
     bool waited = (S == 1);
-    RING_DBG_DECL;
     for (int it = 0; it < items; ++it) {
-      RING_CLK(t0);
       if (use > 0) {
         if (!waited) cluster_wait(), waited = true;
         mbar_wait(&empty[slot], (uint32_t)((use - 1) & 1));
       }
-      RING_CLK(t1);
-      RING_ACC(0, t1 - t0);
       const int g0 = kg_lo + j * kSlotGroups, ng = min(kSlotGroups, kg_hi - g0);
       const int n0 = (o_lo + 2 * rb) * 8, nch = min(16, o_hi * 8 - n0);
       uint8_t* sw = ring + slot * kSlotBytes;
@@ -276,24 +240,15 @@ __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __gri
                           (pw ? szb : scb) + ((size_t)(g0 + grp) * N + n0 + half * 8) * 2);
       }
       ring_cp_async_arrive(&full[slot]);
-      RING_CLK(t2);
-      RING_ACC(1, t2 - t1);
-      RING_ACC(3, 1);
       if (++j == nsl) j = 0, ++rb;
       if (++slot == NS) slot = 0, ++use;
     }
     if (!waited) cluster_wait();
-    if (pw == 0) {
-      RING_STAMP(1);
-    }
-    RING_DBG_FLUSH(warp);
     return;
   }
 
   if (S > 1) cluster_wait();
-  RING_STAMP(2);
   pdl_wait_prior_grid();  // activations (and y) belong to the stream order from here on
-  RING_STAMP(3);
 
   if (warp == kRingCons + kRingProd) {
     // ------------------------------------------------------------------ finisher: cross-warp sum, k-split exchange, y
@@ -337,7 +292,6 @@ __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __gri
         }
       }
     }
-    RING_STAMP(6);
     return;
   }
 
@@ -365,14 +319,12 @@ __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __gri
           *reinterpret_cast<uint32_t*>(d + 128) = v.z;
           *reinterpret_cast<uint32_t*>(d + 192) = v.w;
         }
-        if (MODE == 2) {
+        if constexpr (MODE == 2) {
           const uint32_t w[4] = {v.x, v.y, v.z, v.w};
           float f = 0.f;
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
-            float2 p;
-            if constexpr (kBf16) p = __bfloat1622float2(u32_as_b2(w[e]));
-            else p = __half22float2(u32_as_h2(w[e]));
+            const float2 p = __half22float2(u32_as_h2(w[e]));
             f += p.x + p.y;
           }
           // 16 consecutive lanes = one group; even chunks sit on low-nibble positions (pairs j = 0, 2), odd on high
@@ -382,7 +334,7 @@ __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __gri
           const float o = __shfl_xor_sync(0xffffffffu, f, 1);
           if (ok && (c & 15) == 0) {
             const float lo = f, hi = o, X = lo + hi;
-            xsum[tok * L.ngr + (c >> 4)] = make_float2(X, kBf16 ? 128.f * X : 1024.f * lo + 64.f * hi);
+            xsum[tok * L.ngr + (c >> 4)] = make_float2(X, 1024.f * lo + 64.f * hi);
           }
         }
       }
@@ -391,7 +343,6 @@ __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __gri
       for (int i = tid + M * L.ngr; i < 8 * L.ngr; i += kRingCons * 32) xsum[i] = make_float2(0.f, 0.f);
   }
   consumer_bar();
-  RING_STAMP(4);
 
   // ldmatrix row address of this lane: matrix m = lane >> 3 is the 32-k block, row = channel (lane & 7) of the octet
   const int lm = lane >> 3, lg = lane & 7;
@@ -404,41 +355,33 @@ __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __gri
   for (int i = 0; i < 16; ++i) xq[i] = 0u;
 
   int slot = 0, use = 0;
-  RING_DBG_DECL;
   for (int rb = 0; rb < nrb; ++rb) {
     const int n0 = (o_lo + 2 * rb) * 8;
     const bool two = (o_hi * 8 - n0) >= 16;  // second octet present
     float yacc[4] = {0.f, 0.f, 0.f, 0.f}, yacc2[4] = {0.f, 0.f, 0.f, 0.f};
     for (int j = 0; j < nsl; ++j) {
-      RING_CLK(t0);
       mbar_wait(&full[slot], (uint32_t)(use & 1));
-      RING_CLK(t1);
-      RING_ACC(0, t1 - t0);
       const int ng = min(kSlotGroups, ngr - j * kSlotGroups);
       const uint32_t sb = ring_u32 + (uint32_t)slot * kSlotBytes;
 #pragma unroll
       for (int step = 0; step < 2; ++step) {
         const int gi = warp + kRingCons * step;
-        if (gi < ng && !RING_DRY) {
+        if (gi < ng) {
           const int Gl = j * kSlotGroups + gi;
           const uint32_t wsrc = sb + ldsm_off + step * (kRingCons * 256);
           const uint32_t xsrc = x_u32 + (uint32_t)Gl * 256u;
           const uint32_t ssrc = sb + kSlotW + (uint32_t)(gi * 32 + g * 2);
           const float2* csrc = xsum + (2 * tig) * L.ngr + Gl;
-          if (two) group_step<T, MODE, M1, true>(wsrc, xsrc, ssrc, csrc, L.ngr, live, xq, yacc, yacc2);
-          else group_step<T, MODE, M1, false>(wsrc, xsrc, ssrc, csrc, L.ngr, live, xq, yacc, yacc2);
+          if (two) group_step<T, M1, true>(wsrc, xsrc, ssrc, csrc, L.ngr, live, xq, yacc, yacc2);
+          else group_step<T, M1, false>(wsrc, xsrc, ssrc, csrc, L.ngr, live, xq, yacc, yacc2);
         }
       }
-      RING_CLK(t2);
-      RING_ACC(1, t2 - t1);
-      RING_ACC(3, 1);
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[slot]);  // the slot's words are in registers / consumed
       if (++slot == NS) slot = 0, ++use;
     }
     // this warp's partial sums of the row block -> red[rb & 1][warp]; the finisher adds the 8 warps
     const int rs = rb & 1;
-    RING_CLK(t3);
     if (rb >= 2) mbar_wait(&rbfree[rs], (uint32_t)(((rb >> 1) - 1) & 1));
     if (MODE == 0) {
 #pragma unroll
@@ -449,22 +392,8 @@ __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __gri
     *reinterpret_cast<float2*>(r + (g + 8) * 8 + 2 * tig) = make_float2(yacc[2], yacc[3]);
     __syncwarp();
     if (lane == 0) mbar_arrive(&rbfull[rs]);
-    RING_CLK(t4);
-    RING_ACC(2, t4 - t3);
   }
-  RING_STAMP(5);
-  RING_DBG_FLUSH(warp);
 }
-
-
-#ifdef B200AWQ_TRACE
-extern "C" int b200awq_debug_ring_stats(long long* host) {
-  return (int)cudaMemcpyFromSymbol(host, g_ring_dbg, sizeof(long long) * 80);
-}
-extern "C" int b200awq_debug_ring_flags(int flags) {
-  return (int)cudaMemcpyToSymbol(g_ring_dbg_flags, &flags, sizeof(int));
-}
-#endif
 
 // ------------------------------------------------------------------------------------ host
 namespace {
@@ -482,16 +411,11 @@ int sm_count() {
   return cnt[dev];
 }
 
-int next_ring_seq() {
-  static int seq = 0;
-  return seq++;
-}
-
 constexpr int kRingSmemBudget = 113 * 1024;  // two CTAs (+ 1 KB reserved each) per 228 KB SM
 
-template <typename T, int MODE, bool M1>
+template <typename T, bool M1>
 int launch_ring_t(const RingArgs& a, bool pdl, cudaStream_t stream) {
-  auto kern = w4a16_ring_kernel<T, MODE, M1>;
+  auto kern = w4a16_ring_kernel<T, M1>;
   static bool attr_set[32] = {};
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return B200AWQ_ERR_DEVICE;
@@ -528,7 +452,7 @@ int launch_ring_t(const RingArgs& a, bool pdl, cudaStream_t stream) {
 }  // namespace
 
 int launch_ring(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                bool pdl, const RingTuning& tune, cudaStream_t stream) {
+                bool pdl, cudaStream_t stream) {
   if (M < 1 || M > 8 || N % 8 || K % kGroup) return B200AWQ_ERR_SHAPE;
   const int nsm = sm_count();
   if (nsm < 2) return B200AWQ_ERR_SHAPE;
@@ -536,19 +460,13 @@ int launch_ring(const void* x, const void* qw, const void* sc, const void* sz, v
   RingArgs a{};
   a.x = x, a.qw = static_cast<const uint16_t*>(qw), a.sc = sc, a.sz = sz, a.y = y;
   a.M = M, a.N = N, a.K = K;
-  a.S = (tune.split == 1 || tune.split == 2) ? tune.split : ((G >= 2 * kRingCons && nsm % 2 == 0) ? 2 : 1);
-  if (a.S == 2 && (G < 2 || nsm % 2)) a.S = 1;
+  a.S = (G >= 2 * kRingCons && nsm % 2 == 0) ? 2 : 1;
   a.units = nsm / a.S;
   a.Mp = M <= 1 ? 1 : (M <= 2 ? 2 : (M <= 4 ? 4 : 8));
-  a.seq = next_ring_seq();
   const int oct_max = (O + a.units - 1) / a.units;
   const int nrb_max = (oct_max + 1) / 2;
   if (nrb_max > kRingMaxRb) return B200AWQ_ERR_SHAPE;
-  a.nrb_max = nrb_max;
   const int ngr = (G + a.S - 1) / a.S;
-  // arithmetic: fp16 -> group-factored fp16 MACs (MODE 2); bf16 -> operand-exact (MODE 0).  (One fp16 token normally
-  // never gets here: w4a16_decode.cu serves it.)
-  const int mode = (tune.mode == 0 || tune.mode == 2) ? tune.mode : (dtype == B200AWQ_DTYPE_F16 ? 2 : 0);
   RingLayout& L = a.L;
   L.ngr = ngr;
   L.xrow = ngr * 256;
@@ -561,20 +479,14 @@ int launch_ring(const void* x, const void* qw, const void* sc, const void* sz, v
   L.xchg = off, off += nrb_max * 16 * a.Mp * 4;
   off = (off + 127) & ~127;
   L.ring = off;
-  int ns = (kRingSmemBudget - off) / kSlotBytes;
-  if (tune.slots > 0) ns = std::min(ns, tune.slots);
-  ns = std::min(ns, 8);
+  const int ns = std::min((kRingSmemBudget - off) / kSlotBytes, 8);
   if (ns < 3) return B200AWQ_ERR_SHAPE;  // activations too large next to a useful ring: the caller falls back
   a.NS = ns;
   L.total = off + ns * kSlotBytes;
   const bool m1 = (M == 1);
-  if (dtype == B200AWQ_DTYPE_F16) {
-    if (mode == 0) return m1 ? launch_ring_t<__half, 0, true>(a, pdl, stream) : launch_ring_t<__half, 0, false>(a, pdl, stream);
-    return m1 ? launch_ring_t<__half, 2, true>(a, pdl, stream) : launch_ring_t<__half, 2, false>(a, pdl, stream);
-  }
-  if (mode == 0)
-    return m1 ? launch_ring_t<__nv_bfloat16, 0, true>(a, pdl, stream) : launch_ring_t<__nv_bfloat16, 0, false>(a, pdl, stream);
-  return m1 ? launch_ring_t<__nv_bfloat16, 2, true>(a, pdl, stream) : launch_ring_t<__nv_bfloat16, 2, false>(a, pdl, stream);
+  if (dtype == B200AWQ_DTYPE_F16)
+    return m1 ? launch_ring_t<__half, true>(a, pdl, stream) : launch_ring_t<__half, false>(a, pdl, stream);
+  return m1 ? launch_ring_t<__nv_bfloat16, true>(a, pdl, stream) : launch_ring_t<__nv_bfloat16, false>(a, pdl, stream);
 }
 
 }  // namespace b200awq

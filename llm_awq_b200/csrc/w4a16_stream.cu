@@ -27,22 +27,21 @@
 //     memory, and across the CTAs of a thread-block cluster (split-K for large k)
 //     through distributed shared memory.  No global atomics, no workspace.
 //
-// MODE 0: operands w~ = rn_T(q*s + z) bit-identical to the reference's (13 ALU ops per 8
-//         weights).  Default for bf16, where operand rounding (2^-9) is part of the 1e-3 contract.
-// MODE 2: raw biased operands straight out of the LOP3 (1024+q for low nibbles | 64+q for high
-//         nibbles in fp16, 128+q for bf16; 5 ALU ops per 8 weights); scale, zero and the bias are
-//         applied per 128-k group in fp32:
-//             y += s*(acc - C) + z*X,   X = sum_k x_k,  C = 1024*X_lo + 64*X_hi  (bf16: 128*X).
-//         Exact in the integer q; differs from MODE 0 only by not rounding q*s+z to T.
-//         Default for fp16 (that rounding is 2^-12 relative: ~2e-4 normwise, inside 1e-3).
+// The arithmetic follows the dtype:
+// MODE 0 (bf16): operands w~ = rn_T(q*s + z) bit-identical to the reference's (13 ALU ops per 8
+//         weights): for bf16, operand rounding (2^-9) is part of the 1e-3 contract.
+// MODE 2 (fp16): raw biased operands straight out of the LOP3 (1024+q for low nibbles | 64+q for
+//         high nibbles; 5 ALU ops per 8 weights); scale, zero and the bias are applied per 128-k
+//         group in fp32:
+//             y += s*(acc - C) + z*X,   X = sum_k x_k,  C = 1024*X_lo + 64*X_hi.
+//         Exact in the integer q; differs from MODE 0 only by not rounding q*s+z to T
+//         (that rounding is 2^-12 relative: ~2e-4 normwise, inside 1e-3).
 #include <algorithm>
-#include <atomic>
 
 #include "w4_common.cuh"
 #include "w4a16_kernels.h"
 
 namespace b200awq {
-
 
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
   unsigned long long t;
@@ -56,43 +55,33 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
 constexpr unsigned long long kExchangeTimeoutNs = 10ull * 1000 * 1000 * 1000;
 __device__ unsigned int g_exchange_dead = 0;
 
-#ifdef B200AWQ_TRACE
-// Debug build only (-DB200AWQ_TRACE): wall-clock stamps of the first and last CTA of each launch.
-__device__ unsigned long long g_trace_buf[1024 * 2 * 8];
-#define B200AWQ_STAMP(ev)                                                     \
-  if (threadIdx.x == 0 && (blockIdx.x == 0 || blockIdx.x == gridDim.x - 1)) \
-  g_trace_buf[(((unsigned)seq & 1023u) * 2 + (blockIdx.x != 0)) * 8 + (ev)] = globaltimer_ns()
-#else
-#define B200AWQ_STAMP(ev)
-#endif
+constexpr int kStreamWarps = 8;   // per CTA; each owns the groups g % 8 == warp of the CTA's k range
+constexpr int kStreamRpb = 64;    // 1024-k rounds per prefetch barrier (copy = 2 kStreamRpb KB): one barrier per CTA
 
 struct StreamSmem {
   int w, s, z, x, red, cpart, rbuf, xsum, bars, total;
   int ngroups, nrounds, nbar;  // derived on the host so the kernel prologue has no integer divisions
-  int rbs;                     // row blocks (of 8*RO channels) this CTA processes one after the other
 };
 
-__host__ __device__ inline StreamSmem stream_smem_layout(int RO, int TT, int MODE, int M, int Kc, int rpb, int rbs, int kStreamWarps,
-                                                         bool split) {
+inline StreamSmem stream_smem_layout(int RO, int TT, int MODE, int M, int Kc, bool split) {
   StreamSmem L;
   const int ng = Kc / kGroup;
-  const int nbar = ((ng + kStreamWarps - 1) / kStreamWarps + rpb - 1) / rpb;
+  const int nbar = ((ng + kStreamWarps - 1) / kStreamWarps + kStreamRpb - 1) / kStreamRpb;
   int off = 0;
-  L.w = off, off += rbs * 2 * RO * Kc * 2;
-  L.s = off, off += rbs * ng * 8 * RO * 2;
-  L.z = off, off += rbs * ng * 8 * RO * 2;
+  L.w = off, off += 2 * RO * Kc * 2;
+  L.s = off, off += ng * 8 * RO * 2;
+  L.z = off, off += ng * 8 * RO * 2;
   off = (off + 15) & ~15;
   L.x = off, off += M * (Kc * 2 + 16);
   L.red = off, off += kStreamWarps * TT * 128 * 4;
   L.cpart = off, off += TT * 128 * 4;
   L.rbuf = off, off += (split ? 8 * TT * 128 * 4 : 0);  // split-k: partial sums pushed by the other CTAs of the cluster
   L.xsum = off, off += (MODE ? 8 * TT * ng * 8 : 0);
-  L.bars = off, off += (rbs * nbar + 2) * 8;
+  L.bars = off, off += (nbar + 2) * 8;
   L.total = off;
   L.ngroups = ng;
   L.nrounds = (ng + kStreamWarps - 1) / kStreamWarps;
   L.nbar = nbar;
-  L.rbs = rbs;
   return L;
 }
 
@@ -101,13 +90,12 @@ __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src)
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
-template <typename T, int RO, int TT, int MODE, int kStreamWarps>
-__global__ void __launch_bounds__(kStreamWarps * 32, TT == 1 ? (kStreamWarps == 16 ? 2 : 4) : (kStreamWarps == 16 ? 1 : 2))
+template <typename T, int RO, int TT>
+__global__ void __launch_bounds__(kStreamWarps * 32, TT == 1 ? 4 : 2)
 w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, const T* __restrict__ scales,
-                    const T* __restrict__ szeros, T* __restrict__ y, int M, int N, int K, int Kc, int S, int rpb, int seq,
+                    const T* __restrict__ szeros, T* __restrict__ y, int M, int N, int K, int Kc, int S,
                     const __grid_constant__ StreamSmem L, const __grid_constant__ PeerArgs pa) {
-  B200AWQ_STAMP(0);
-  constexpr bool kBf16 = TypeTraits<T>::kIsBf16;
+  constexpr int MODE = TypeTraits<T>::kIsBf16 ? 0 : 2;  // see the header comment
   constexpr int R = 8 * RO;  // output channels per CTA
   constexpr int kStreamThreads = kStreamWarps * 32;
   constexpr int kRoundK = kStreamWarps * kGroup;  // input channels consumed per round of the warps
@@ -115,8 +103,8 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31, g = lane >> 2, tig = lane & 3;
   const int rank = (S > 1) ? (int)cluster_ctarank() : 0;
-  const int rb0 = ((S > 1) ? (int)(blockIdx.x / S) : (int)blockIdx.x) * L.rbs;  // first row block of this CTA
-  const int rbs = min(L.rbs, N / R - rb0);                                      // (the last CTA may own fewer)
+  const int rb = (S > 1) ? (int)(blockIdx.x / S) : (int)blockIdx.x;  // row block (of R channels) of this CTA
+  const int n0 = rb * R;
   const int kbase = rank * Kc;
   const int ngroups = L.ngroups, nrounds = L.nrounds, nbar = L.nbar;
   const int wrow = Kc * 2;       // bytes of one 4-row quad over this CTA's k range
@@ -130,58 +118,50 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
   float* cpart = reinterpret_cast<float*>(smem + L.cpart);  // [tt][16][8]
   float2* xsum = reinterpret_cast<float2*>(smem + L.xsum);  // [8 TT tok][group] {X, C}   (MODE 2)
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bars);
-  uint64_t* xbar = bars + L.rbs * nbar;
+  uint64_t* xbar = bars + nbar;
   uint64_t* rbar = xbar + 1;                                 // split-k: counts the bytes pushed into rbuf
   float* rbuf = reinterpret_cast<float*>(smem + L.rbuf);    // [cluster rank][tt][16][8]
 
   if (tid == 0) {
-    for (int b = 0; b <= L.rbs * nbar + 1; ++b) mbar_init(&bars[b], 1);
+    for (int b = 0; b <= nbar + 1; ++b) mbar_init(&bars[b], 1);
     mbar_fence_init();
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    B200AWQ_STAMP(7);
   }
   pdl_launch_dependents();
   // ---- scales / zeros of this CTA's rows and groups -> shared memory, asynchronously (16-byte pieces)
   {
     constexpr int PPG = R / 8;  // 16-byte pieces per group per tensor
     const int pieces = ngroups * PPG;
-    for (int rbi = 0; rbi < rbs; ++rbi) {
-      const size_t goff = ((size_t)(kbase / kGroup) * N + (size_t)(rb0 + rbi) * R) * 2;
-      const uint8_t* sg = reinterpret_cast<const uint8_t*>(scales) + goff;
-      const uint8_t* zg = reinterpret_cast<const uint8_t*>(szeros) + goff;
-      for (int i = tid; i < 2 * pieces; i += kStreamThreads) {
-        const int which = i >= pieces;
-        const int j = which ? i - pieces : i;
-        const int grp = j / PPG, pc = j - grp * PPG;
-        cp_async16(reinterpret_cast<uint8_t*>(which ? zbuf : sbuf) + ((rbi * ngroups + grp) * PPG + pc) * 16,
-                   (which ? zg : sg) + (size_t)grp * N * 2 + pc * 16);
-      }
+    const size_t goff = ((size_t)(kbase / kGroup) * N + (size_t)n0) * 2;
+    const uint8_t* sg = reinterpret_cast<const uint8_t*>(scales) + goff;
+    const uint8_t* zg = reinterpret_cast<const uint8_t*>(szeros) + goff;
+    for (int i = tid; i < 2 * pieces; i += kStreamThreads) {
+      const int which = i >= pieces;
+      const int j = which ? i - pieces : i;
+      const int grp = j / PPG, pc = j - grp * PPG;
+      cp_async16(reinterpret_cast<uint8_t*>(which ? zbuf : sbuf) + (grp * PPG + pc) * 16,
+                 (which ? zg : sg) + (size_t)grp * N * 2 + pc * 16);
     }
-    if (MODE) {  // tokens M .. 8*TT-1 do not exist: their correction terms must read as zero
+    if constexpr (MODE == 2) {  // tokens M .. 8*TT-1 do not exist: their correction terms must read as zero
       for (int i = tid + M * ngroups; i < 8 * TT * ngroups; i += kStreamThreads) xsum[i] = make_float2(0.f, 0.f);
     }
   }
   __syncthreads();  // barrier inits and the zeroed correction terms visible to everyone
-  // ---- weight prefetch: 2*RO quad rows (x rbs row blocks) x nbar pieces of (rpb * 1024 k) each, one bulk copy per
-  // (quad row, piece); the copies of different quad rows are issued by different warps (a single thread needs
-  // ~0.15 us per cp.async.bulk: measured 0.64 us for four of them)
+  // ---- weight prefetch: 2*RO quad rows x nbar pieces of (kStreamRpb * 1024 k) each, one bulk copy per (quad row,
+  // piece); the copies of different quad rows are issued by different warps (a single thread needs ~0.15 us per
+  // cp.async.bulk: measured 0.64 us for four of them)
   if (lane == 0 && warp < 2 * RO) {
-    const int piece = rpb * kRoundK * 2;  // bytes per quad row per barrier
-    for (int rbi = 0; rbi < rbs; ++rbi)
-      for (int b = 0; b < nbar; ++b) {
-        const int off = b * piece;
-        const int len = min(piece, wrow - off);
-        if (warp == 0) mbar_expect_tx(&bars[rbi * nbar + b], 2 * RO * len);
-        bulk_g2s(wbuf + (rbi * 2 * RO + warp) * wrow + off,
-                 reinterpret_cast<const uint8_t*>(qw + (size_t)((rb0 + rbi) * 2 * RO + warp) * K + kbase) + off, len,
-                 &bars[rbi * nbar + b]);
-      }
+    constexpr int piece = kStreamRpb * kRoundK * 2;  // bytes per quad row per barrier
+    for (int b = 0; b < nbar; ++b) {
+      const int off = b * piece;
+      const int len = min(piece, wrow - off);
+      if (warp == 0) mbar_expect_tx(&bars[b], 2 * RO * len);
+      bulk_g2s(wbuf + warp * wrow + off, reinterpret_cast<const uint8_t*>(qw + (size_t)(rb * 2 * RO + warp) * K + kbase) + off,
+               len, &bars[b]);
+    }
   }
-  B200AWQ_STAMP(1);
   if (S > 1) cluster_sync_all();  // ... and to the other CTAs of the cluster, BEFORE the wait (overlaps the previous kernel)
-  B200AWQ_STAMP(2);
   pdl_wait_prior_grid();  // activations (and y) belong to the stream order from here on
-  B200AWQ_STAMP(3);
 
   // ---- activations: M bulk copies x[m, kbase .. kbase + Kc) -> xbuf (natural order)
   if (tid == 0) {
@@ -189,7 +169,7 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
     for (int m = 0; m < M; ++m) bulk_g2s(xbuf + m * xrow, x + (size_t)m * K + kbase, Kc * 2, xbar);
   }
   mbar_wait(xbar, 0);
-  if (MODE) {
+  if constexpr (MODE == 2) {
     // {X, C} of (token, group) for THIS warp's groups only (nobody else reads them): lane = (group
     // slot, 16-element chunk); the first 16 B of a chunk sit on low-nibble positions, the second on
     // high-nibble ones (pairs 0-3 | 4-7 of each half of the 32-k block).
@@ -204,14 +184,7 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
           const uint32_t av[4] = {va.x, va.y, va.z, va.w}, bv[4] = {vb.x, vb.y, vb.z, vb.w};
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
-            float2 fa, fb;
-            if constexpr (kBf16) {
-              fa = __bfloat1622float2(u32_as_b2(av[e]));
-              fb = __bfloat1622float2(u32_as_b2(bv[e]));
-            } else {
-              fa = __half22float2(u32_as_h2(av[e]));
-              fb = __half22float2(u32_as_h2(bv[e]));
-            }
+            const float2 fa = __half22float2(u32_as_h2(av[e])), fb = __half22float2(u32_as_h2(bv[e]));
             lo += fa.x + fa.y;
             hi += fb.x + fb.y;
           }
@@ -223,7 +196,7 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
         }
         if (chunk == 0 && G < ngroups) {
           const float X = lo + hi;
-          xsum[m * ngroups + G] = make_float2(X, kBf16 ? 128.f * X : 1024.f * lo + 64.f * hi);
+          xsum[m * ngroups + G] = make_float2(X, 1024.f * lo + 64.f * hi);
         }
       }
     }
@@ -231,11 +204,8 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
   }
   cp_async_wait_all();  // scales / zeros (issued before the wait; their latency overlapped everything above)
   __syncthreads();
-  B200AWQ_STAMP(4);
 
   const float zero4[4] = {0.f, 0.f, 0.f, 0.f};
-  for (int rbi = 0; rbi < rbs; ++rbi) {  // row blocks of this CTA: weights of all of them were prefetched above
-  const int n0 = (rb0 + rbi) * R;
   float acc[TT][4];
 #pragma unroll
   for (int t = 0; t < TT; ++t)
@@ -251,9 +221,9 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
     live[t] = tok < M;
     xp[t] = xbuf + (live[t] ? tok : 0) * xrow + (warp * kGroup + tig * 32) * 2;
   }
-  const uint8_t* wp = wbuf + (rbi * 2 * RO + (g >> 2)) * wrow + (warp * 2 + (tig >> 1)) * 128 + (g & 3) * 32 + (tig & 1) * 16;
-  const uint16_t* sq = sbuf + (rbi * ngroups + warp) * R + g;
-  const uint16_t* zq = zbuf + (rbi * ngroups + warp) * R + g;
+  const uint8_t* wp = wbuf + (g >> 2) * wrow + (warp * 2 + (tig >> 1)) * 128 + (g & 3) * 32 + (tig & 1) * 16;
+  const uint16_t* sq = sbuf + warp * R + g;
+  const uint16_t* zq = zbuf + warp * R + g;
   const float2* sump = xsum + (2 * tig) * ngroups + warp;  // token 2 tig (+ 8 t), this warp's first group
   uint4 xq[TT][4];
 #pragma unroll
@@ -261,10 +231,10 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
 #pragma unroll
     for (int j = 0; j < 4; ++j) xq[t][j] = make_uint4(0, 0, 0, 0);
 
-  for (int rnd = 0, G = warp, left = 0, bar = rbi * nbar; rnd < nrounds; ++rnd, G += kStreamWarps) {
+  for (int rnd = 0, G = warp, left = 0, bar = 0; rnd < nrounds; ++rnd, G += kStreamWarps) {
     if (left == 0) {
       mbar_wait(&bars[bar++], 0);
-      left = rpb;
+      left = kStreamRpb;
     }
     --left;
     if (G >= ngroups) break;  // only in the last round, when ngroups % 8 != 0
@@ -301,7 +271,7 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
       // words uu, uu+1 of both octets; the MMA of nibble pair j takes (word uu, word uu+1) as its two
       // k slots, so its B operand is the ADJACENT register pair (4j + uu, 4j + uu + 1) of xq[j]
       uint32_t oa0[4], oa1[4], ob0[4] = {0, 0, 0, 0}, ob1[4] = {0, 0, 0, 0};
-      if (MODE == 0) {
+      if constexpr (MODE == 0) {
         dequant_word<T>(wa[uu], sa2, za2, oa0);
         dequant_word<T>(wa[uu + 1], sa2, za2, oa1);
         if (RO == 2) {
@@ -309,11 +279,11 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
           dequant_word<T>(wb[uu + 1], sb2, zb2, ob1);
         }
       } else {
-        unpack_word_biased<T>(wa[uu], oa0);
-        unpack_word_biased<T>(wa[uu + 1], oa1);
+        unpack_word_biased(wa[uu], oa0);
+        unpack_word_biased(wa[uu + 1], oa1);
         if (RO == 2) {
-          unpack_word_biased<T>(wb[uu], ob0);
-          unpack_word_biased<T>(wb[uu + 1], ob1);
+          unpack_word_biased(wb[uu], ob0);
+          unpack_word_biased(wb[uu + 1], ob1);
         }
       }
 #pragma unroll
@@ -321,7 +291,7 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           const uint32_t b0 = uu ? xq[t][j].z : xq[t][j].x, b1 = uu ? xq[t][j].w : xq[t][j].y;
-          if (MODE == 0) {
+          if constexpr (MODE == 0) {
             mma_16816<T>(acc[t], oa0[j], ob0[j], oa1[j], ob1[j], b0, b1, acc[t]);
           } else {
             // two independent accumulation chains (even / odd j); low-nibble pairs are j = 0, 2
@@ -334,10 +304,10 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
         }
       }
     }
-    if (MODE) {
+    if constexpr (MODE == 2) {
       // part[t][0..1]: (row g of octet 0, tokens 8t + 2tig, + 1); part[t][2..3]: row g of octet 1
-      const float sa = bits16_to_float(s_a, kBf16), za = bits16_to_float(z_a, kBf16);
-      const float sb = bits16_to_float(s_b, kBf16), zb = bits16_to_float(z_b, kBf16);
+      const float sa = half_bits_to_float(s_a), za = half_bits_to_float(z_a);
+      const float sb = half_bits_to_float(s_b), zb = half_bits_to_float(z_b);
 #pragma unroll
       for (int t = 0; t < TT; ++t) {
         const float2 c0 = sump[(8 * t) * ngroups], c1 = sump[(8 * t + 1) * ngroups];  // {X, C}, zeros if absent
@@ -350,7 +320,6 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
     }
   }
 
-  B200AWQ_STAMP(5);
   // acc[t][0..1]: (channel g, tokens 8t + 2tig, +1); acc[t][2..3]: channel 8 + g
 #pragma unroll
   for (int t = 0; t < TT; ++t) {
@@ -391,7 +360,7 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
       }
     } else {
       if (tid == 0) mbar_expect_tx(rbar, (uint32_t)((S - 1) * nvalid * 4));
-      mbar_wait(rbar, (uint32_t)(rbi & 1));
+      mbar_wait(rbar, 0);
       for (int e = tid; e < TT * 128; e += kStreamThreads) {
         const int t = e >> 7, row = (e >> 3) & 15, tok = 8 * t + (e & 7);
         if (tok < M && row < R) {
@@ -460,31 +429,13 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
     __syncthreads();
     if (tid < R / 8) pa.epoch[idx + tid] = s_ep[tid];
   }
-  if (rbi + 1 < rbs) __syncthreads();  // `red` / `cpart` are reused by the next row block
-  }  // rbi
-  B200AWQ_STAMP(6);
 }
-
-#ifdef B200AWQ_TRACE
-extern "C" int b200awq_debug_read_trace(unsigned long long* host, int count) {
-  return (int)cudaMemcpyFromSymbol(host, g_trace_buf, sizeof(unsigned long long) * (size_t)count);
-}
-#endif
 
 // ------------------------------------------------------------------------------------ host
 constexpr int kStreamSmemCap = 200 * 1024;
 
-static int next_seq() {  // launch counter for the trace build's stamps only
-  static std::atomic<int> seq{0};
-  return seq.fetch_add(1, std::memory_order_relaxed);
-}
-
-static int pick_splits(int K, int kc_target, int kc_env) {
+static int pick_splits(int K, int kc_target) {
   const int groups = K / kGroup;
-  if (kc_env > 0 && kc_env % kGroup == 0 && K % kc_env == 0) {
-    const int s = K / kc_env;
-    if (s == 1 || s == 2 || s == 4 || s == 8) return s;
-  }
   int best = 1;
   for (int s = 1; s <= 8; s *= 2) {  // cluster sizes: powers of two, <= 8 (portable limit)
     if (groups % s) continue;
@@ -494,42 +445,34 @@ static int pick_splits(int K, int kc_target, int kc_env) {
   return best;
 }
 
-template <typename T, int RO, int TT, int MODE, int kStreamWarps>
-static int launch_stream_w(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K,
-                           int S, int rpb, bool pdl, const StreamTuning& tune, cudaStream_t stream, const PeerArgs* peers) {
+// One row block of 8 RO channels per CTA: several per CTA (prefetched up front, activations staged once) would make
+// fat long-lived CTAs that keep the NEXT launch's CTAs from becoming resident, which costs more than the saved prologues.
+template <typename T, int RO, int TT>
+static int launch_stream_t(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K,
+                           int S, bool pdl, cudaStream_t stream, const PeerArgs* peers) {
+  constexpr int MODE = TypeTraits<T>::kIsBf16 ? 0 : 2;
   const int Kc = K / S;
   PeerArgs pa{};
   if (peers) pa = *peers;
   if (pa.world > 1 && TT != 1) return B200AWQ_ERR_SHAPE;
-  // several row blocks per CTA (all weight slices prefetched up front, activations / group sums staged once) is a
-  // tuning knob only: fat long-lived CTAs keep the NEXT launch's CTAs from becoming resident, which costs more
-  // than the saved prologues
-  const int nblk = N / (8 * RO);
-  int rbs = (tune.rbs > 0) ? tune.rbs : 1;
-  if (S != 1 || rbs > nblk) rbs = 1;
-  StreamSmem L = stream_smem_layout(RO, TT, MODE, M, Kc, rpb, rbs, kStreamWarps, S > 1);
-  if (L.total > kStreamSmemCap && rbs > 1) rbs = 1, L = stream_smem_layout(RO, TT, MODE, M, Kc, rpb, 1, kStreamWarps, S > 1);
+  const StreamSmem L = stream_smem_layout(RO, TT, MODE, M, Kc, S > 1);
   if (L.total > kStreamSmemCap) return B200AWQ_ERR_SHAPE;
-  constexpr int kStreamThreads = kStreamWarps * 32;
-  auto kern = w4a16_stream_kernel<T, RO, TT, MODE, kStreamWarps>;
+  auto kern = w4a16_stream_kernel<T, RO, TT>;
   static bool attr_set[32] = {};  // per kernel instantiation and device
   if (cudaError_t ea = ensure_dyn_smem(kern, kStreamSmemCap, attr_set)) return (int)ea;
+  const int ctas = N / (8 * RO) * S;
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)((nblk + rbs - 1) / rbs) * S);
-  cfg.blockDim = dim3(kStreamThreads);
+  cfg.gridDim = dim3((unsigned)ctas);
+  cfg.blockDim = dim3(kStreamWarps * 32);
   // Co-residency: a launch that fits in one wave runs fastest with FEW CTAs per SM (the next launch's
   // CTAs only need enough room to prefetch); multi-wave launches want as many as fit (measured, DESIGN.md).
   size_t dyn = L.total;
-  const int ctas = ((nblk + rbs - 1) / rbs) * S;
   int dev = 0, nsm = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
   if (nsm <= 0) nsm = 132;
   const int per_sm = ctas <= 2 * nsm ? 2 : (ctas <= 3 * nsm ? 3 : 0);
-  if (tune.pad > 0)  // > 0: explicit extra bytes (limits co-residency), 0: heuristic, < 0: none
-    dyn += (size_t)tune.pad;
-  else if (tune.pad == 0 && per_sm > 0 && S == 1)
-    dyn = std::max(dyn, (size_t)(233472 / (per_sm + 1) - 512));
+  if (per_sm > 0 && S == 1) dyn = std::max(dyn, (size_t)(233472 / (per_sm + 1) - 512));
   if (dyn > (size_t)kStreamSmemCap) dyn = L.total;
   cfg.dynamicSmemBytes = dyn;
   cfg.stream = stream;
@@ -550,48 +493,31 @@ static int launch_stream_w(const void* x, const void* qw, const void* sc, const 
   cfg.attrs = attrs;
   cfg.numAttrs = na;
   cudaError_t e = cudaLaunchKernelEx(&cfg, kern, (const T*)x, (const uint16_t*)qw, (const T*)sc, (const T*)sz, (T*)y, M, N,
-                                     K, Kc, S, rpb, next_seq(), L, pa);
+                                     K, Kc, S, L, pa);
   return e == cudaSuccess ? 0 : (int)e;
 }
 
-template <typename T, int RO, int TT, int MODE>
-static int launch_stream_t(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K,
-                           int S, int rpb, bool pdl, const StreamTuning& tune, cudaStream_t stream, const PeerArgs* peers) {
-  // 8 warps per CTA by default; 16 (shorter serial chain after griddepcontrol.wait, half the co-residency) is a knob
-  if (tune.warps == 16)  // 16 warps or several row blocks per CTA do not pay
-    return launch_stream_w<T, RO, TT, MODE, 16>(x, qw, sc, sz, y, M, N, K, S, rpb, pdl, tune, stream, peers);
-  return launch_stream_w<T, RO, TT, MODE, 8>(x, qw, sc, sz, y, M, N, K, S, rpb, pdl, tune, stream, peers);
-}
-
-template <typename T, int MODE>
+template <typename T>
 static int launch_stream_m(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K,
-                           int S, int ro, int rpb, bool pdl, const StreamTuning& tune, cudaStream_t stream,
-                           const PeerArgs* peers) {
+                           int S, int ro, bool pdl, cudaStream_t stream, const PeerArgs* peers) {
   if (M <= 8) {
-    if (ro == 2) return launch_stream_t<T, 2, 1, MODE>(x, qw, sc, sz, y, M, N, K, S, rpb, pdl, tune, stream, peers);
-    return launch_stream_t<T, 1, 1, MODE>(x, qw, sc, sz, y, M, N, K, S, rpb, pdl, tune, stream, peers);
+    if (ro == 2) return launch_stream_t<T, 2, 1>(x, qw, sc, sz, y, M, N, K, S, pdl, stream, peers);
+    return launch_stream_t<T, 1, 1>(x, qw, sc, sz, y, M, N, K, S, pdl, stream, peers);
   }
-  if (ro == 2) return launch_stream_t<T, 2, 2, MODE>(x, qw, sc, sz, y, M, N, K, S, rpb, pdl, tune, stream, peers);
-  return launch_stream_t<T, 1, 2, MODE>(x, qw, sc, sz, y, M, N, K, S, rpb, pdl, tune, stream, peers);
+  if (ro == 2) return launch_stream_t<T, 2, 2>(x, qw, sc, sz, y, M, N, K, S, pdl, stream, peers);
+  return launch_stream_t<T, 1, 2>(x, qw, sc, sz, y, M, N, K, S, pdl, stream, peers);
 }
 
 int launch_stream(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                  bool pdl, const StreamTuning& tune, cudaStream_t stream, const PeerArgs* peers) {
+                  bool pdl, cudaStream_t stream, const PeerArgs* peers) {
   if (M < 1 || M > 16 || N % 8 || K % kGroup) return B200AWQ_ERR_SHAPE;
   const int ro = (N % 16 == 0) ? 2 : 1;
   // k per CTA: splitting k over a cluster doubles the CTAs and adds the cluster reduction; up to 4 tokens the unsplit
   // 4096 rather than 2048, above that shared memory for x decides
   const int kc_target = M <= 4 ? 4096 : (M <= 8 ? 2048 : 1024);
-  const int S = pick_splits(K, kc_target, tune.kc);
-  const int rpb = tune.rpb > 0 ? tune.rpb : 64;  // default: one barrier (4 large copies) per CTA
-  // default arithmetic: fp16 -> group-factored (MODE 2), bf16 -> operand-exact (MODE 0); see the header comment
-  const int mode = (tune.mode == 0 || tune.mode == 2) ? tune.mode : (dtype == B200AWQ_DTYPE_F16 ? 2 : 0);
-  if (dtype == B200AWQ_DTYPE_F16) {
-    if (mode == 0) return launch_stream_m<__half, 0>(x, qw, sc, sz, y, M, N, K, S, ro, rpb, pdl, tune, stream, peers);
-    return launch_stream_m<__half, 2>(x, qw, sc, sz, y, M, N, K, S, ro, rpb, pdl, tune, stream, peers);
-  }
-  if (mode == 0) return launch_stream_m<__nv_bfloat16, 0>(x, qw, sc, sz, y, M, N, K, S, ro, rpb, pdl, tune, stream, peers);
-  return launch_stream_m<__nv_bfloat16, 2>(x, qw, sc, sz, y, M, N, K, S, ro, rpb, pdl, tune, stream, peers);
+  const int S = pick_splits(K, kc_target);
+  if (dtype == B200AWQ_DTYPE_F16) return launch_stream_m<__half>(x, qw, sc, sz, y, M, N, K, S, ro, pdl, stream, peers);
+  return launch_stream_m<__nv_bfloat16>(x, qw, sc, sz, y, M, N, K, S, ro, pdl, stream, peers);
 }
 
 }  // namespace b200awq

@@ -425,55 +425,45 @@ static int launch_wgmma(int tn, const void* x, const void* qw, const void* sc, c
 }
 
 int launch_umma(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                bool pdl, const UmmaTuning& tune, cudaStream_t stream) {
+                bool pdl, cudaStream_t stream) {
   if (M < 1 || N % kBM || K % kGroup) return B200AWQ_ERR_SHAPE;
   const int sms = wg_sm_count();
-  int tn = tune.tn;
-  int split = tune.split;
-  if (tn != 16 && tn != 32 && tn != 64 && tn != 128) {
-    // joint choice of the token tile and the k split by a small cost model (cycles per CTA, estimated): a 64-k stage
-    // costs max(dequantisation ~400, wgmma 4 * tn + 100), a tile's epilogue ~10 tn (+6000 when the partial tiles of
-    // a split are reduced over the cluster), a launch ~12000; makespan = waves x that
-    long best = -1;
-    for (int c = 128; c >= 16; c >>= 1) {
-      if (c > 16 && c / 2 >= M) continue;
-      const int tiles = ((M + c - 1) / c) * (N / kBM);
-      for (int sp = 1; sp <= 8; sp *= 2) {
-        if (sp > 1 && (c > 64 || (K / kGroup) % sp || K / sp < 512 || tune.split == 1)) continue;
-        if (tune.split > 1 && sp != tune.split && c <= 64) continue;
-        const long per_tile = (long)(K / kBK / sp) * (4 * c + 100 > 400 ? 4 * c + 100 : 400) + 10 * c + (sp > 1 ? 6000 : 0);
-        const long slots = sms / sp;  // clusters that run at once
-        const long cost = 12000 + ((tiles + slots - 1) / slots) * per_tile;
-        if (best < 0 || cost < best) best = cost, tn = c, split = sp;
-      }
+  // joint choice of the token tile and the k split by a small cost model (cycles per CTA, estimated): a 64-k stage
+  // costs max(dequantisation ~400, wgmma 4 * tn + 100), a tile's epilogue ~10 tn (+6000 when the partial tiles of
+  // a split are reduced over the cluster), a launch ~12000; makespan = waves x that.  A split (cluster of S CTAs on
+  // one tile) needs tn <= 64, S dividing the group count and >= 512 k per CTA.
+  int tn = 16, S = 1;
+  long best = -1;
+  for (int c = 128; c >= 16; c >>= 1) {
+    if (c > 16 && c / 2 >= M) continue;
+    const int tiles = ((M + c - 1) / c) * (N / kBM);
+    for (int sp = 1; sp <= 8; sp *= 2) {
+      if (sp > 1 && (c > 64 || (K / kGroup) % sp || K / sp < 512)) continue;
+      const long per_tile = (long)(K / kBK / sp) * (4 * c + 100 > 400 ? 4 * c + 100 : 400) + 10 * c + (sp > 1 ? 6000 : 0);
+      const long slots = sms / sp;  // clusters that run at once
+      const long cost = 12000 + ((tiles + slots - 1) / slots) * per_tile;
+      if (best < 0 || cost < best) best = cost, tn = c, S = sp;
     }
   }
-  int S = 1;
-  if (tn <= 64 && split > 1 && split <= 8 && (split & (split - 1)) == 0 && (K / kGroup) % split == 0) S = split;
-  int ctas = sms;
-  if (tune.max_ctas > 0 && tune.max_ctas < ctas) ctas = tune.max_ctas;
-  return launch_wgmma(tn, x, qw, sc, sz, y, M, N, K, dtype, pdl, ctas / S > 0 ? ctas / S : 1, S, stream);
+  // a persistent grid of one CTA per SM
+  return launch_wgmma(tn, x, qw, sc, sz, y, M, N, K, dtype, pdl, sms / S > 0 ? sms / S : 1, S, stream);
 }
 
 // Skinny batches (HBM-bound): one 16-token tile, one CTA per 128 output channels and k slice, every CTA resident at
 // once so that several stream their weights per SM.  The k split is the smallest (<= 8, dividing the group count)
 // whose slice is <= 512 k, or <= 1024 k once there are at least two CTAs per SM.
 int launch_flat(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                bool pdl, const FlatTuning& tune, cudaStream_t stream) {
+                bool pdl, cudaStream_t stream) {
   if (M < 1 || M > 64 || N % kBM || K % kGroup) return B200AWQ_ERR_SHAPE;
   const int groups = K / kGroup;
+  const int sms = wg_sm_count();
   int S = 1;
-  if (tune.kc > 0 && tune.kc % kGroup == 0 && K % tune.kc == 0 && K / tune.kc <= 8) {
-    S = K / tune.kc;
-  } else {
-    const int sms = wg_sm_count();
-    for (int s = 1; s <= 8; ++s) {
-      if (groups % s) continue;
-      S = s;
-      const int kc = K / s;
-      if (kc <= 512) break;
-      if (kc <= 1024 && (N / kBM) * s >= 2 * sms) break;
-    }
+  for (int s = 1; s <= 8; ++s) {
+    if (groups % s) continue;
+    S = s;
+    const int kc = K / s;
+    if (kc <= 512) break;
+    if (kc <= 1024 && (N / kBM) * s >= 2 * sms) break;
   }
   const int tn = M <= 16 ? 16 : (M <= 32 ? 32 : 64);
   return launch_wgmma(tn, x, qw, sc, sz, y, M, N, K, dtype, pdl, 0, S, stream);
