@@ -168,6 +168,25 @@ int b200awq_rotary_embedding_neox(const long long* positions, void* query, void*
                                   int q_heads, int k_heads, int head_size, int rot_dim, long long q_token_stride,
                                   long long k_token_stride, int dtype, void* stream);
 
+/* Forward attention over many queries (prefill, vision towers).  Replaces flash-attn 2's flash_attn_func and
+ * flash_attn_varlen_qkvpacked_func (called from tinychat/modules/fused_attn.py, models/llama.py, models/qwen2.py,
+ * modules/fused_siglipdecoder.py and models/internvl/internvit.py) for the parameters those callers pass:
+ *   out = softmax(softmax_scale * q k^T + mask) v per (sequence, query head); query head h reads KV head
+ *   h / (heads / kv_heads).  causal != 0 aligns the mask bottom-right: query i sees keys j <= i + Sk - Sq; a row that
+ *   sees no key is zero.  S in fp32 from T operands, softmax in fp32, P rounded to T, O in fp32 rounded once to T.
+ * q [.., Sq, H, D], k / v [.., Sk, Hkv, D]: strides in ELEMENTS for (batch, token, head), unit element stride;
+ * out [batch * Sq or total_q, H, D] contiguous.  cu_seqlens_q / cu_seqlens_k: NULL for fixed lengths, else batch + 1
+ * int32 offsets into the token dimension in DEVICE memory, read by the kernel only (batch strides ignored; seqlen_q /
+ * seqlen_k are then the maxima).  head_dim in {64, 72, 128}, heads % kv_heads == 0 and a finite softmax_scale > 0
+ * (else B200AWQ_ERR_SHAPE);
+ * q, k, v, out 16-byte aligned and strides multiples of 8 elements (else B200AWQ_ERR_ALIGN).  seqlen_q == 0 or
+ * batch == 0 is a no-op.  Deterministic: no split over keys, no atomics, no workspace. */
+int b200awq_prefill_attention(const void* q, const void* k, const void* v, void* out,
+                              const int* cu_seqlens_q, const int* cu_seqlens_k,
+                              int batch, int seqlen_q, int seqlen_k, int heads, int kv_heads, int head_dim,
+                              const long long q_strides[3], const long long k_strides[3], const long long v_strides[3],
+                              float softmax_scale, int causal, int dtype, void* stream);
+
 /* ---- W8A8 (int8 weights, int8 per-token activations): the vision-tower ops of the reference's extension
  * (csrc/pybind.cpp:30-37), called by awq/quantize/w8a8_linear.py and tinychat's QuantSiglipEncoder /
  * QuantInternVisionEncoder.  Scales are fp16 everywhere (the reference reads them as at::Half).  fp32 activations,

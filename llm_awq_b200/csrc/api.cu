@@ -2,6 +2,7 @@
 // between the HBM-bound streaming kernels and the wgmma tensor-core kernel, the PDL switch.
 // No torch types, no allocation, no synchronisation.
 #include <atomic>
+#include <cmath>
 #include <cstdint>
 #include <cstdlib>
 #include <initializer_list>
@@ -200,6 +201,29 @@ int b200awq_single_query_attention(const void* q, const void* k, const void* v, 
                                                        rotary_base,
                                                        rotary_scale, neox, dtype, workspace, workspace_bytes, pdl_enabled(),
                                                        static_cast<cudaStream_t>(stream));
+  if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
+  return r;
+}
+
+int b200awq_prefill_attention(const void* q, const void* k, const void* v, void* out, const int* cu_seqlens_q,
+                              const int* cu_seqlens_k, int batch, int seqlen_q, int seqlen_k, int heads, int kv_heads,
+                              int head_dim, const long long q_strides[3], const long long k_strides[3],
+                              const long long v_strides[3], float softmax_scale, int causal, int dtype, void* stream) {
+  if (dtype != B200AWQ_DTYPE_F16 && dtype != B200AWQ_DTYPE_BF16) return B200AWQ_ERR_DTYPE;
+  if (batch < 0 || seqlen_q < 0 || seqlen_k < 0 || heads < 1 || kv_heads < 1 || heads % kv_heads ||
+      (head_dim != 64 && head_dim != 72 && head_dim != 128) || !(std::isfinite(softmax_scale) && softmax_scale > 0.f))
+    return B200AWQ_ERR_SHAPE;  // the softmax runs on the raw scores' max: scale > 0
+  if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(out) || !q_strides || !k_strides || !v_strides)
+    return B200AWQ_ERR_ALIGN;
+  if ((cu_seqlens_q == nullptr) != (cu_seqlens_k == nullptr)) return B200AWQ_ERR_ALIGN;
+  for (const long long* s : {q_strides, k_strides, v_strides})
+    for (int i = 0; i < 3; ++i)
+      if (s[i] % 8) return B200AWQ_ERR_ALIGN;  // TMA takes 16-byte strides
+  if (int e = check_device()) return e;
+  if (batch == 0 || seqlen_q == 0) return 0;
+  const int r = b200awq::launch_prefill_attention(q, k, v, out, cu_seqlens_q, cu_seqlens_k, batch, seqlen_q, seqlen_k, heads,
+                                                  kv_heads, head_dim, q_strides, k_strides, v_strides, softmax_scale, causal != 0,
+                                                  dtype, static_cast<cudaStream_t>(stream));
   if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
   return r;
 }

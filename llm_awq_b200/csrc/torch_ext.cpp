@@ -381,6 +381,79 @@ void gelu_and_quant(torch::Tensor& out, torch::Tensor& input, torch::Tensor& sca
         false);
 }
 
+// ---------------------------------------------------------------- attention over many queries
+// flash-attn 2.8.3's flash_attn_func / flash_attn_varlen_qkvpacked_func (flash_attn/flash_attn_interface.py): same
+// names, positional order and keyword names for the parameters tinychat's callers pass.  Like flash-attn, an operand
+// whose last dimension is not contiguous, or whose strides or pointer the TMA cannot take, is copied contiguous first;
+// views into a fused qkv buffer are used in place.
+namespace {
+
+torch::Tensor tma_ready(const torch::Tensor& t) {
+  const bool ok = t.stride(-1) == 1 && (reinterpret_cast<uintptr_t>(t.data_ptr()) & 15u) == 0 &&
+                  t.stride(0) % 8 == 0 && t.stride(1) % 8 == 0 && t.stride(2) % 8 == 0;
+  return ok ? t : t.clone(at::MemoryFormat::Contiguous);  // a fresh allocation: aligned, dense strides
+}
+
+void check_attention_args(const torch::Tensor& q, const torch::Tensor& k, const torch::Tensor& v, double dropout_p,
+                          const char* fn) {
+  TORCH_CHECK(q.is_cuda() && k.is_cuda() && v.is_cuda(), fn, ": q, k, v must be CUDA tensors");
+  TORCH_CHECK(dropout_p == 0.0, fn, ": dropout is not supported by this build (dropout_p must be 0)");
+  TORCH_CHECK(q.scalar_type() == at::ScalarType::Half || q.scalar_type() == at::ScalarType::BFloat16, fn,
+              ": only fp16 and bf16 are supported");
+  TORCH_CHECK(k.scalar_type() == q.scalar_type() && v.scalar_type() == q.scalar_type(), fn,
+              ": query and key / value must have the same dtype");
+}
+
+torch::Tensor run_prefill_attention(const torch::Tensor& q_in, const torch::Tensor& k_in, const torch::Tensor& v_in,
+                                    torch::Tensor& out, const int* cu_seqlens, int batch, int seqlen_q, int seqlen_k,
+                                    c10::optional<double> softmax_scale, bool causal) {
+  const c10::cuda::CUDAGuard guard(q_in.device());
+  const torch::Tensor q = tma_ready(q_in), k = tma_ready(k_in), v = tma_ready(v_in);
+  const int heads = q.size(-2), kv_heads = k.size(-2), d = q.size(-1);
+  const float scale = softmax_scale.has_value() ? (float)softmax_scale.value() : 1.0f / std::sqrt((float)d);
+  const long long qs[3] = {q.stride(0), q.stride(1), q.stride(2)};
+  const long long ks[3] = {k.stride(0), k.stride(1), k.stride(2)};
+  const long long vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
+  raise(b200awq_prefill_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), cu_seqlens, cu_seqlens, batch,
+                                  seqlen_q, seqlen_k, heads, kv_heads, d, qs, ks, vs, scale, causal ? 1 : 0,
+                                  q.scalar_type() == at::ScalarType::Half ? B200AWQ_DTYPE_F16 : B200AWQ_DTYPE_BF16,
+                                  at::cuda::getCurrentCUDAStream().stream()),
+        false);
+  return out;
+}
+
+}  // namespace
+
+// q [B, Sq, H, D], k / v [B, Sk, Hkv, D] -> out [B, Sq, H, D]
+torch::Tensor flash_attn_func(const torch::Tensor& q, const torch::Tensor& k, const torch::Tensor& v, double dropout_p,
+                              c10::optional<double> softmax_scale, bool causal) {
+  const char* fn = "flash_attn_func";
+  check_attention_args(q, k, v, dropout_p, fn);
+  TORCH_CHECK(q.dim() == 4 && k.dim() == 4 && v.dim() == 4, fn, ": q, k, v must be [batch, seqlen, heads, head_dim]");
+  TORCH_CHECK(k.sizes() == v.sizes(), fn, ": k and v must have the same shape");
+  TORCH_CHECK(k.size(0) == q.size(0) && k.size(3) == q.size(3), fn, ": k / v batch and head_dim must match q");
+  torch::Tensor out = torch::empty(q.sizes(), q.options());
+  return run_prefill_attention(q, k, v, out, nullptr, q.size(0), q.size(1), k.size(1), softmax_scale, causal);
+}
+
+// qkv [total, 3, H, D], cu_seqlens int32 [batch + 1] -> out [total, H, D]
+torch::Tensor flash_attn_varlen_qkvpacked_func(const torch::Tensor& qkv, const torch::Tensor& cu_seqlens, int64_t max_seqlen,
+                                               double dropout_p, c10::optional<double> softmax_scale, bool causal) {
+  const char* fn = "flash_attn_varlen_qkvpacked_func";
+  TORCH_CHECK(qkv.dim() == 4 && qkv.size(1) == 3, fn, ": qkv must be [total_tokens, 3, heads, head_dim]");
+  const torch::Tensor q = qkv.select(1, 0), k = qkv.select(1, 1), v = qkv.select(1, 2);
+  check_attention_args(q, k, v, dropout_p, fn);
+  TORCH_CHECK(cu_seqlens.is_cuda() && cu_seqlens.scalar_type() == at::ScalarType::Int && cu_seqlens.dim() == 1 &&
+                  cu_seqlens.is_contiguous() && cu_seqlens.numel() >= 1,
+              fn, ": cu_seqlens must be a contiguous int32 CUDA tensor [batch + 1]");
+  TORCH_CHECK(cu_seqlens.device() == qkv.device(), fn, ": cu_seqlens must be on qkv's device");
+  TORCH_CHECK(max_seqlen >= 0 && max_seqlen <= INT32_MAX, fn, ": bad max_seqlen");
+  torch::Tensor out = torch::empty({qkv.size(0), qkv.size(2), qkv.size(3)}, qkv.options());
+  // [total, H, D] views as [1, total, H, D]: the batch stride is ignored for packed sequences
+  return run_prefill_attention(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), out, cu_seqlens.data_ptr<int>(),
+                               (int)cu_seqlens.numel() - 1, (int)max_seqlen, (int)max_seqlen, softmax_scale, causal);
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "H100 (sm_90a) drop-in for llm-awq's awq_inference_engine (W4A16 and W8A8 paths)";
   m.def("gemm_forward_cuda_new", &gemm_forward_cuda_new, "New quantized GEMM kernel.");
@@ -402,6 +475,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         "LayerNorm + int8 quantization (per token or per tensor)");
   m.def("silu_and_mul", &silu_and_mul, "Activation function.");
   m.def("gelu_and_quant", &gelu_and_quant, "Apply gelu act and quant output");
+  m.def("flash_attn_func", &flash_attn_func, "Attention over many queries (flash-attn's flash_attn_func)", py::arg("q"),
+        py::arg("k"), py::arg("v"), py::arg("dropout_p") = 0.0, py::arg("softmax_scale") = py::none(),
+        py::arg("causal") = false);
+  m.def("flash_attn_varlen_qkvpacked_func", &flash_attn_varlen_qkvpacked_func,
+        "Attention over packed sequences of a fused qkv tensor (flash-attn's flash_attn_varlen_qkvpacked_func)",
+        py::arg("qkv"), py::arg("cu_seqlens"), py::arg("max_seqlen"), py::arg("dropout_p") = 0.0,
+        py::arg("softmax_scale") = py::none(), py::arg("causal") = false);
   m.def("set_pdl", [](bool on) { return b200awq_set_pdl(on ? 1 : 0) != 0; }, "programmatic dependent launch on/off");
   m.def("launch_count", []() { return b200awq_launch_count(); }, "kernels launched by libb200awq so far");
   m.def("version", []() { return std::string(b200awq_version()); });

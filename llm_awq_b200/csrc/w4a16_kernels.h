@@ -83,6 +83,12 @@ int launch_rope_neox(const long long* positions, void* query, void* key, const v
                      int k_heads, int head_size, int rot_dim, long long q_stride, long long k_stride, int dtype, bool pdl,
                      cudaStream_t stream);
 
+// forward attention over many queries, D in {64, 72, 128}; arguments as b200awq_prefill_attention (prefill_attention.cu)
+int launch_prefill_attention(const void* q, const void* k, const void* v, void* out, const int* cu_q, const int* cu_k, int batch,
+                             int seqlen_q, int seqlen_k, int heads, int kv_heads, int head_dim, const long long* q_strides,
+                             const long long* k_strides, const long long* v_strides, float softmax_scale, bool causal, int dtype,
+                             cudaStream_t stream);
+
 // the same kernel for skinny batches, 1 <= M <= 64, N % 128 == 0: one CTA per tile and k slice (w4a16_wgmma.cu)
 int launch_flat(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
                 bool pdl, cudaStream_t stream);
