@@ -187,6 +187,27 @@ int b200awq_prefill_attention(const void* q, const void* k, const void* v, void*
                               const long long q_strides[3], const long long k_strides[3], const long long v_strides[3],
                               float softmax_scale, int causal, int dtype, void* stream);
 
+/* Attention of few queries over many keys (long-context decode, few-token chunks): flash_attn_func's fixed-length
+ * call as tinychat's long_forward makes it (tinychat/modules/fused_attn.py, q [B, 1, H, D] over views
+ * cache[:, :start_pos + 1] of [B, Lmax, Hkv, D] caches), with the key range split over CTAs.  Same semantics, layouts,
+ * strides, alignment rules and return codes as b200awq_prefill_attention for fixed lengths (no cu_seqlens), within a
+ * narrower envelope: head_dim in {64, 128} and seqlen_q * (heads / kv_heads) <= 64 (else B200AWQ_ERR_SHAPE; callers
+ * fall through to b200awq_prefill_attention).  k / v are read only for tokens < seqlen_k, whatever lies past them.
+ * `workspace`: >= b200awq_splitkv_attention_workspace_bytes(...) bytes of 16-byte aligned device memory (else
+ * B200AWQ_ERR_WORKSPACE), ZERO before the first use, then owned by the kernel, which leaves its counters zero; one
+ * workspace per stream.  The workspace of b200awq_single_query_attention on the same stream may serve both (their
+ * counters share one block at offset 0).  A size of 0 means no workspace is needed (NULL is fine): the shape always
+ * runs as one split (one 128-key tile, or batch * kv_heads > 4096, more cells than the counter block holds).  A CUDA
+ * graph that captured a call keeps using the workspace it captured: it must stay allocated, and zero in its counter
+ * block, for as long as the graph is replayed (the launches leave it so).  Deterministic: the splits are combined in a fixed order, no atomics in the arithmetic. */
+int b200awq_splitkv_attention(const void* q, const void* k, const void* v, void* out,
+                              int batch, int seqlen_q, int seqlen_k, int heads, int kv_heads, int head_dim,
+                              const long long q_strides[3], const long long k_strides[3], const long long v_strides[3],
+                              float softmax_scale, int causal, int dtype, void* workspace, size_t workspace_bytes,
+                              void* stream);
+size_t b200awq_splitkv_attention_workspace_bytes(int batch, int seqlen_q, int seqlen_k, int heads, int kv_heads,
+                                                 int head_dim);
+
 /* ---- W8A8 (int8 weights, int8 per-token activations): the vision-tower ops of the reference's extension
  * (csrc/pybind.cpp:30-37), called by awq/quantize/w8a8_linear.py and tinychat's QuantSiglipEncoder /
  * QuantInternVisionEncoder.  Scales are fp16 everywhere (the reference reads them as at::Half).  fp32 activations,

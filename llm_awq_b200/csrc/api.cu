@@ -228,6 +228,37 @@ int b200awq_prefill_attention(const void* q, const void* k, const void* v, void*
   return r;
 }
 
+size_t b200awq_splitkv_attention_workspace_bytes(int batch, int seqlen_q, int seqlen_k, int heads, int kv_heads, int head_dim) {
+  return b200awq::splitkv_attention_workspace_bytes(batch, seqlen_q, seqlen_k, heads, kv_heads, head_dim);
+}
+
+int b200awq_splitkv_attention(const void* q, const void* k, const void* v, void* out, int batch, int seqlen_q, int seqlen_k,
+                              int heads, int kv_heads, int head_dim, const long long q_strides[3],
+                              const long long k_strides[3], const long long v_strides[3], float softmax_scale, int causal,
+                              int dtype, void* workspace, size_t workspace_bytes, void* stream) {
+  if (dtype != B200AWQ_DTYPE_F16 && dtype != B200AWQ_DTYPE_BF16) return B200AWQ_ERR_DTYPE;
+  if (batch < 0 || seqlen_q < 0 || seqlen_k < 0 || heads < 1 || kv_heads < 1 || heads % kv_heads ||
+      (long long)seqlen_q * (heads / kv_heads) > 64 || (head_dim != 64 && head_dim != 128) ||
+      !(std::isfinite(softmax_scale) && softmax_scale > 0.f))
+    return B200AWQ_ERR_SHAPE;  // the softmax runs on the raw scores' max: scale > 0
+  if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(out) || !q_strides || !k_strides || !v_strides)
+    return B200AWQ_ERR_ALIGN;
+  for (const long long* s : {q_strides, k_strides, v_strides})
+    for (int i = 0; i < 3; ++i)
+      if (s[i] % 8) return B200AWQ_ERR_ALIGN;  // TMA takes 16-byte strides; Q is read in 16-byte pieces
+  if (workspace && !aligned16(workspace)) return B200AWQ_ERR_ALIGN;
+  if (workspace_bytes < b200awq::splitkv_attention_workspace_bytes(batch, seqlen_q, seqlen_k, heads, kv_heads, head_dim) ||
+      (workspace_bytes && !workspace))
+    return B200AWQ_ERR_WORKSPACE;
+  if (int e = check_device()) return e;
+  if (batch == 0 || seqlen_q == 0) return 0;
+  const int r = b200awq::launch_splitkv_attention(q, k, v, out, batch, seqlen_q, seqlen_k, heads, kv_heads, head_dim, q_strides,
+                                                  k_strides, v_strides, softmax_scale, causal != 0, dtype, workspace,
+                                                  workspace_bytes, static_cast<cudaStream_t>(stream));
+  if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
+  return r;
+}
+
 int b200awq_rope_with_pos(const void* x, const float* freqs, void* y, int s, int b, int h, int d, int d2,
                           const long long in_strides[4], const long long out_strides[4], int dtype, void* stream) {
   if (dtype != B200AWQ_DTYPE_F16 && dtype != B200AWQ_DTYPE_BF16) return B200AWQ_ERR_DTYPE;

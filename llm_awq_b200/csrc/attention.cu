@@ -47,7 +47,7 @@ __device__ __forceinline__ void unpack8(const uint4& v, float (&f)[8]) {
 constexpr int kAttThreads = 256;
 constexpr int kAttMaxGS = 8;   // query heads per CTA (a head group); G = H / Hkv > 8 takes ceil(G / 8) groups
 constexpr int kAttMaxD = 256;  // head dimension
-constexpr int kAttCounters = 4096;  // batch * kv_heads * groups the workspace's counter block is sized for
+constexpr int kAttCounters = kAttentionCounters;  // batch * kv_heads * groups the workspace's counter block is sized for
 
 // Head groups of a KV head: ceil(G / 8) groups of near-equal size gs = ceil(G / groups) <= 8; the last group's heads
 // past G are masked.  For G <= 8: one group of G heads.

@@ -9,9 +9,11 @@
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
 
+#include <algorithm>
 #include <initializer_list>
 #include <map>
 #include <stdexcept>
+#include <vector>
 
 #include "../../include/b200awq.h"
 
@@ -148,6 +150,32 @@ void layernorm_forward_cuda(torch::Tensor _input, torch::Tensor _gamma, torch::T
         false);
 }
 
+namespace {
+
+// The attention workspace of the current stream on `like`'s device, at least `need` bytes: one zero-initialised buffer
+// per (device, stream), shared by single_query_attention and the split-key attention behind flash_attn_func (their
+// counter blocks coincide and every launch leaves its counters zero).  When a call needs more, a new zeroed buffer of
+// at least twice the size takes over, and the ones it replaces are kept, never freed: a CUDA graph that captured a call
+// on this stream keeps launching with the buffer it captured, which must stay valid (its counters stay zero, since
+// every launch leaves them so).  The doubling bounds how many buffers are kept.
+// Leaked on purpose: CUDA tensors must not be destroyed by static destructors at interpreter exit.
+const torch::Tensor& attention_workspace(const torch::Tensor& like, size_t need) {
+  struct Buffers {
+    torch::Tensor current;
+    std::vector<torch::Tensor> replaced;  // still referenced by graphs captured before a growth
+  };
+  static auto& workspaces = *new std::map<std::pair<int, void*>, Buffers>();
+  Buffers& w = workspaces[std::make_pair((int)like.get_device(), (void*)at::cuda::getCurrentCUDAStream().stream())];
+  const size_t have = w.current.defined() ? (size_t)w.current.numel() : 0;
+  if (have < need) {
+    if (w.current.defined()) w.replaced.push_back(w.current);
+    w.current = torch::zeros({(int64_t)std::max(need, 2 * have)}, like.options().dtype(torch::kUInt8));
+  }
+  return w.current;
+}
+
+}  // namespace
+
 // reference: awq/kernels/csrc/attention/ft_attention.cpp:112-184 (same checks, same argument order and defaults,
 // pybind.cpp:24-27).  alibi_slopes must be None; fp32 tensors are not dispatched.  Like the reference, any
 // nheads % nheads_kv == 0 and any headdim % 8 == 0 up to 256 run.
@@ -180,21 +208,13 @@ torch::Tensor single_query_attention(const torch::Tensor q, const torch::Tensor 
   }
   const c10::cuda::CUDAGuard guard(q.device());
   torch::Tensor out = torch::empty({batch_size, nheads, headdim}, q.options());
-  // one zero-initialised workspace per (device, stream); the kernels leave it zero where it matters
-  // (leaked on purpose: CUDA tensors must not be destroyed by static destructors at interpreter exit)
-  static auto& workspaces = *new std::map<std::pair<int, void*>, torch::Tensor>();
-  const size_t need = b200awq_single_query_attention_workspace_bytes(batch_size, nheads, nheads_kv, headdim, memory_max_seqlen);
-  void* st = at::cuda::getCurrentCUDAStream().stream();
-  auto key = std::make_pair((int)q.get_device(), st);
-  auto it = workspaces.find(key);
-  if (it == workspaces.end() || (size_t)it->second.numel() < need) {
-    workspaces[key] = torch::zeros({(int64_t)need}, q.options().dtype(torch::kUInt8));
-    it = workspaces.find(key);
-  }
+  const torch::Tensor& ws = attention_workspace(
+      q, b200awq_single_query_attention_workspace_bytes(batch_size, nheads, nheads_kv, headdim, memory_max_seqlen));
   raise(b200awq_single_query_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
                                        out.data_ptr(), lps, batch_size, nheads, nheads_kv, headdim, memory_max_seqlen, timestep,
                                        (long long)q.stride(0), (long long)k.stride(0), (long long)v.stride(0), rotary_embedding_dim, rotary_base, rotary_scale,
-                                       neox_rotary_style ? 1 : 0, dt, it->second.data_ptr(), (size_t)it->second.numel(), st),
+                                       neox_rotary_style ? 1 : 0, dt, ws.data_ptr(), (size_t)ws.numel(),
+                                       at::cuda::getCurrentCUDAStream().stream()),
         false);
   return out;
 }
@@ -383,7 +403,8 @@ void gelu_and_quant(torch::Tensor& out, torch::Tensor& input, torch::Tensor& sca
 
 // ---------------------------------------------------------------- attention over many queries
 // flash-attn 2.8.3's flash_attn_func / flash_attn_varlen_qkvpacked_func (flash_attn/flash_attn_interface.py): same
-// names, positional order and keyword names for the parameters tinychat's callers pass.  Like flash-attn, an operand
+// names, positional order and keyword names for the parameters tinychat's callers pass.  Fixed-length calls with few
+// queries per KV head (decode over a long context) take the split-key kernel, everything else the prefill kernel.  Like flash-attn, an operand
 // whose last dimension is not contiguous, or whose strides or pointer the TMA cannot take, is copied contiguous first;
 // views into a fused qkv buffer are used in place.
 namespace {
@@ -414,11 +435,20 @@ torch::Tensor run_prefill_attention(const torch::Tensor& q_in, const torch::Tens
   const long long qs[3] = {q.stride(0), q.stride(1), q.stride(2)};
   const long long ks[3] = {k.stride(0), k.stride(1), k.stride(2)};
   const long long vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
-  raise(b200awq_prefill_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), cu_seqlens, cu_seqlens, batch,
-                                  seqlen_q, seqlen_k, heads, kv_heads, d, qs, ks, vs, scale, causal ? 1 : 0,
-                                  q.scalar_type() == at::ScalarType::Half ? B200AWQ_DTYPE_F16 : B200AWQ_DTYPE_BF16,
-                                  at::cuda::getCurrentCUDAStream().stream()),
-        false);
+  const int dt = q.scalar_type() == at::ScalarType::Half ? B200AWQ_DTYPE_F16 : B200AWQ_DTYPE_BF16;
+  void* st = at::cuda::getCurrentCUDAStream().stream();
+  int rc = B200AWQ_ERR_SHAPE;
+  if (!cu_seqlens) {  // few queries per KV head: the split-key kernel; outside its envelope the prefill kernel
+    const size_t need = b200awq_splitkv_attention_workspace_bytes(batch, seqlen_q, seqlen_k, heads, kv_heads, d);
+    const torch::Tensor* ws = need ? &attention_workspace(q, need) : nullptr;
+    rc = b200awq_splitkv_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), batch, seqlen_q, seqlen_k, heads,
+                                   kv_heads, d, qs, ks, vs, scale, causal ? 1 : 0, dt, ws ? ws->data_ptr() : nullptr,
+                                   ws ? (size_t)ws->numel() : 0, st);
+  }
+  if (rc == B200AWQ_ERR_SHAPE)
+    rc = b200awq_prefill_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), cu_seqlens, cu_seqlens, batch,
+                                   seqlen_q, seqlen_k, heads, kv_heads, d, qs, ks, vs, scale, causal ? 1 : 0, dt, st);
+  raise(rc, false);
   return out;
 }
 

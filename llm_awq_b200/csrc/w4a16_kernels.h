@@ -70,6 +70,11 @@ int launch_decode_mlp_front(const void* x, const void* gqw, const void* gsc, con
 int launch_silu_mul(const void* gate, const void* up, void* out, size_t rows, size_t cols, size_t in_pitch, int dtype, bool pdl,
                     cudaStream_t stream);
 
+// Both attention workspaces (single-query decode and split-key attention) start with the same block of kAttentionCounters
+// u32 arrival counters, which every launch leaves zero, so that one zero-initialised buffer per stream can serve both:
+// the partials of one entry never alias the other's counters.
+constexpr int kAttentionCounters = 4096;
+
 // single-query (decode-step) attention over tinychat's KV-cache layout + RoPE over [s, b, h, d] (attention.cu)
 size_t attention_workspace_bytes(int batch, int heads, int kv_heads, int head_dim, int max_len);
 int launch_single_query_attention(const void* q, const void* k, const void* v, void* k_cache, void* v_cache, void* out,
@@ -88,6 +93,14 @@ int launch_prefill_attention(const void* q, const void* k, const void* v, void* 
                              int seqlen_q, int seqlen_k, int heads, int kv_heads, int head_dim, const long long* q_strides,
                              const long long* k_strides, const long long* v_strides, float softmax_scale, bool causal, int dtype,
                              cudaStream_t stream);
+
+// attention of few queries over many keys, seqlen_q * (heads / kv_heads) <= 64, D in {64, 128}, split over keys;
+// arguments as b200awq_splitkv_attention (splitkv_attention.cu)
+size_t splitkv_attention_workspace_bytes(int batch, int seqlen_q, int seqlen_k, int heads, int kv_heads, int head_dim);
+int launch_splitkv_attention(const void* q, const void* k, const void* v, void* out, int batch, int seqlen_q, int seqlen_k,
+                             int heads, int kv_heads, int head_dim, const long long* q_strides, const long long* k_strides,
+                             const long long* v_strides, float softmax_scale, bool causal, int dtype, void* workspace,
+                             size_t workspace_bytes, cudaStream_t stream);
 
 // the same kernel for skinny batches, 1 <= M <= 64, N % 128 == 0: one CTA per tile and k slice (w4a16_wgmma.cu)
 int launch_flat(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
