@@ -150,6 +150,25 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
+// The same copy with an L2 eviction priority (`policy`, e.g. from l2_policy_evict_first()).
+__device__ __forceinline__ void bulk_g2s_hint(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar,
+                                              uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+          smem_u32(smem_dst)),
+      "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
+      : "memory");
+}
+// Prefetch of the L2 line holding `gmem_addr` (per lane): no destination, nothing to wait for.
+__device__ __forceinline__ void prefetch_l2(const void* gmem_addr) {
+  asm volatile("prefetch.global.L2 [%0];" ::"l"(gmem_addr));
+}
+// L2 eviction priority of data read once: its lines are the first to be replaced.
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
 
 // ---------------------------------------------------------------- programmatic dependent launch
 __device__ __forceinline__ void pdl_wait_prior_grid() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

@@ -183,6 +183,28 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
     // ------------------------------------------------------------------ producer: weights + scales into the ring
     const uint8_t* scb = reinterpret_cast<const uint8_t*>(a.sc);
     const uint8_t* szb = reinterpret_cast<const uint8_t*>(a.sz);
+    // L2 prefetch of every scale and zero this CTA reads, before the first copy: per group, its quad rows are one span
+    // [q_lo * 8, q_hi * 8) of bytes in a row of each tensor, touched 128 bytes apart and at its last byte, so every
+    // line of the span is fetched and no address leaves the row.  Each slot's 8-byte copies then find their lines in
+    // L2 instead of waiting the full HBM latency.  Per-lane prefetches (one instruction for the warp), not
+    // cp.async.bulk.prefetch: that one takes uniform operands, and 32 different addresses serialise in front of the
+    // first lap.
+    if (nq > 0) {  // (a layer with fewer quad rows than CTAs leaves some CTAs without rows)
+      const uint32_t lo = (uint32_t)q_lo * 8u, hi = (uint32_t)q_hi * 8u;
+      for (int g = kg_lo + lane; g < kg_hi; g += 32) {
+        const size_t row = (size_t)g * N * 2;
+        for (uint32_t o = lo;; o += 128) {
+          const uint32_t at = o < hi ? o : hi - 1;
+          prefetch_l2(scb + row + at);
+          prefetch_l2(szb + row + at);
+          if (FUSED) {
+            prefetch_l2(reinterpret_cast<const uint8_t*>(a.sc2) + row + at);
+            prefetch_l2(reinterpret_cast<const uint8_t*>(a.sz2) + row + at);
+          }
+          if (o >= hi) break;
+        }
+      }
+    }
     int slot = 0, use = 0;
     bool joined = false;  // the CTA barrier is joined once, after the first lap (or at the end of a short walk)
     for (int rb = 0; rb < nrb; ++rb) {
@@ -208,8 +230,10 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
           const uint32_t len = (uint32_t)ng * 256u;
           if (lane == 0) {
             mbar_expect_tx(&full[slot], (uint32_t)nqs * len);
-            bulk_g2s(sw, qwt + (size_t)q0 * K + (size_t)g0 * kGroup, len, &full[slot]);
-            if (nqs > 1) bulk_g2s(sw + kDecQuadB, qwt + (size_t)(q0 + 1) * K + (size_t)g0 * kGroup, len, &full[slot]);
+            const uint64_t policy = l2_policy_evict_first();  // weights are read once: keep L2 for the scales and zeros
+            bulk_g2s_hint(sw, qwt + (size_t)q0 * K + (size_t)g0 * kGroup, len, &full[slot], policy);
+            if (nqs > 1)
+              bulk_g2s_hint(sw + kDecQuadB, qwt + (size_t)(q0 + 1) * K + (size_t)g0 * kGroup, len, &full[slot], policy);
           }
           if (lane < ng) {  // lane = group: 8 bytes (4 channels) of scales and of zeros per quad row
             const size_t off = ((size_t)(g0 + lane) * N + (size_t)q0 * 4) * 2;
