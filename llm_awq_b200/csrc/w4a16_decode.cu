@@ -56,6 +56,47 @@ constexpr int kDecMaxSlots = 8;
 constexpr int kDecMaxRb = 128;                         // row blocks per CTA the exchange buffers are sized for
 constexpr int kDecSmemBudget = 113 * 1024;             // two CTAs (+ 1 KB reserved each) per 228 KB SM
 
+// Handoff of the HBM stream between consecutive launches on one SM (DESIGN §3.1).  g_dec_pending[smid] counts the
+// decode producers on that SM that still have copies to issue.  A producer that arrives while another one is pending
+// issues only kDecHold slots of its first lap, and the rest when the count falls back to its own entry (the other
+// producer issued its last copy, so its bytes in flight are draining) or when its own consumers pass the dependency
+// wait, whichever comes first.  The counters only move that release point: a foreign or stale count delays it to the
+// wait at the latest, which always comes, and no result depends on them.
+constexpr int kDecHold = 2;
+constexpr int kDecMaxSm = 256;  // counters; an SM with a higher id (none on sm_90) never holds
+__device__ unsigned int g_dec_pending[kDecMaxSm];
+
+__device__ __forceinline__ uint32_t dec_smid() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%smid;" : "=r"(r));
+  return r;
+}
+
+#ifdef B200AWQ_DECODE_TRACE
+// Trace build only (bench_decode_trace.py): per-CTA time stamps of the launch-boundary events, read back through
+// b200awq_decode_trace_read().  The product is built without it.
+enum DecTraceEvent { kTrStart, kTrFirstLap, kTrRelease, kTrRefill, kTrLastIssue, kTrWait, kTrLastMac, kTrLastStore };
+struct DecTraceRec {
+  unsigned long long global_ns, clock;
+  const void* layer;  // the launch's weights: tells the layers of a step apart
+  uint32_t block, sm_event;  // sm_event = smid << 8 | event
+};
+constexpr int kDecTraceCap = 1 << 20;
+__device__ DecTraceRec g_dec_trace[kDecTraceCap];
+__device__ unsigned int g_dec_trace_n;
+__device__ __forceinline__ void dec_trace(const void* layer, int event) {
+  unsigned long long t, c;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  asm volatile("mov.u64 %0, %%clock64;" : "=l"(c));
+  if (threadIdx.x & 31) return;  // one record per warp
+  const unsigned int i = atomicAdd(&g_dec_trace_n, 1u);
+  if (i < (unsigned)kDecTraceCap) g_dec_trace[i] = DecTraceRec{t, c, layer, blockIdx.x, dec_smid() << 8 | (uint32_t)event};
+}
+#define DEC_TRACE(layer, event) dec_trace(layer, event)
+#else
+#define DEC_TRACE(layer, event) ((void)0)
+#endif
+
 struct DecLayout {
   int bars, x, gx, red, xchg, ring, total;
 };
@@ -146,7 +187,8 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
   uint64_t* empty = bars + kDecMaxSlots;
   uint64_t* rbfull = bars + 2 * kDecMaxSlots;
   uint64_t* rbfree = rbfull + kDecRed;
-  uint64_t* xch = rbfree + kDecRed;  // [row block] (rank 0 of a cluster)
+  volatile uint32_t* waited = reinterpret_cast<volatile uint32_t*>(rbfree + kDecRed);  // consumers passed the wait
+  uint64_t* xch = rbfree + kDecRed + 1;  // [row block] (rank 0 of a cluster)
   uint8_t* ring = smem + L.ring;
   float* red = reinterpret_cast<float*>(smem + L.red);    // [kDecRed][warp][16 ch]
   float* xchg = reinterpret_cast<float*>(smem + L.xchg);  // [peer 1..S-1][row block][16 ch]: the peers' sums land here (rank 0)
@@ -168,6 +210,7 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
       mbar_init(&rbfull[lane], kDecCons);
       mbar_init(&rbfree[lane], 1);
     }
+    if (lane == 0) *waited = 0u;
     if (S > 1 && rank == 0) {
       for (int rb = lane; rb < nrb; rb += 32) {
         const int nch = min(16, (nq - 4 * rb) * 4);
@@ -205,6 +248,13 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
         }
       }
     }
+    // arrival on this SM's handoff counter; `hold` = slots of the first lap issued before the release
+    const uint32_t sm = dec_smid();
+    unsigned int* pending = sm < (uint32_t)kDecMaxSm ? &g_dec_pending[sm] : nullptr;
+    unsigned int others = 0;
+    if (lane == 0 && pending) others = atomicAdd(pending, 1u);
+    const int hold = __shfl_sync(0xffffffffu, others, 0) != 0u ? kDecHold : NS;
+    DEC_TRACE(a.qw, kTrStart);
     int slot = 0, use = 0;
     bool joined = false;  // the CTA barrier is joined once, after the first lap (or at the end of a short walk)
     for (int rb = 0; rb < nrb; ++rb) {
@@ -217,13 +267,27 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
         const uint8_t* szt = second ? reinterpret_cast<const uint8_t*>(a.sz2) : szb;
         const int g0 = kg_lo + p * kDecPiece, ng = min(kDecPiece, kg_hi - g0);
         for (int h = 0; h < nqb; h += 2) {  // one slot per octet
-          if (use > 0) {
+          if (use > 0 || slot == hold) {
             if (!joined) {
               asm volatile("bar.sync 0;" ::: "memory");  // the CTA barrier the other warps wait at (below)
               if (S > 1) dec_cluster_arrive();
               joined = true;
+              DEC_TRACE(a.qw, kTrFirstLap);
             }
-            mbar_wait(&empty[slot], (uint32_t)((use - 1) & 1));
+            if (use == 0) {
+              // the held part of the first lap: released when the other producer on this SM has issued its last
+              // copy, or when this CTA's consumers have passed the dependency wait
+              for (;;) {
+                unsigned int go = 0;
+                if (lane == 0) go = *waited != 0u || *(volatile unsigned int*)pending <= 1u;
+                if (__shfl_sync(0xffffffffu, go, 0)) break;
+                __nanosleep(128);
+              }
+              DEC_TRACE(a.qw, kTrRelease);
+            } else {
+              mbar_wait(&empty[slot], (uint32_t)((use - 1) & 1));
+              if (use == 1 && slot == 0) DEC_TRACE(a.qw, kTrRefill);
+            }
           }
           const int q0 = qb + h, nqs = min(2, nqb - h);
           uint8_t* sw = ring + slot * kDecSlotBytes;
@@ -250,6 +314,9 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
         }
       }
     }
+    __syncwarp();
+    if (lane == 0 && pending) asm volatile("red.relaxed.gpu.global.add.u32 [%0], %1;" ::"l"(pending), "r"(0xffffffffu) : "memory");
+    DEC_TRACE(a.qw, kTrLastIssue);
     if (!joined) {
       asm volatile("bar.sync 0;" ::: "memory");
       if (S > 1) dec_cluster_arrive();
@@ -279,6 +346,10 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
     for (int i = 0; i < kMaxOwn; ++i) {
       asm volatile("ld.global.u32 %0, [%1];" : "=r"(xa0[i]) : "l"(xfirst[i]) : "memory");
       asm volatile("ld.global.u32 %0, [%1 + 32];" : "=r"(xb0[i]) : "l"(xfirst[i]) : "memory");
+    }
+    if (warp == 0) {
+      if (lane == 0) *waited = 1u;  // releases the producer's held slots if nothing else has
+      DEC_TRACE(a.qw, kTrWait);
     }
   }
 
@@ -351,6 +422,7 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
         finish(r, f0, fch);
       }
     }
+    DEC_TRACE(a.qw, kTrLastStore);
     return;
   }
 
@@ -533,6 +605,7 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
     __syncwarp();
     if (lane == 0) mbar_arrive(&rbfull[rs]);
   }
+  if (warp == 0) DEC_TRACE(a.qw, kTrLastMac);
 }
 
 // ------------------------------------------------------------------------------------ host
@@ -590,11 +663,14 @@ int launch_decode_impl(const void* x, const void* qw, const void* sc, const void
   const int ngr = (G + S - 1) / S;
   DecLayout& L = a.L;
   int off = 0;
-  L.bars = off, off += 8 * (2 * kDecMaxSlots + 2 * kDecRed + kDecMaxRb);
+  // barriers, the `waited` flag and one exchange barrier per row block; `red` holds min(kDecRed, nrb_max) row blocks,
+  // since the kernel indexes both by rb < nrb_max (and red by rb % kDecRed).  Sized to the plan so that the k-split
+  // plan of k = 14336 (4 row blocks per CTA) keeps a 5-slot ring.
+  L.bars = off, off += 8 * (2 * kDecMaxSlots + 2 * kDecRed + 1 + nrb_max);
   off = (off + 127) & ~127;
   L.x = off, off += ngr * kDecGroupBytes;
   L.gx = off, off += ngr * 4 * 4;
-  L.red = off, off += kDecRed * kDecCons * 16 * nt * 4;
+  L.red = off, off += std::min(kDecRed, nrb_max) * kDecCons * 16 * nt * 4;
   L.xchg = off, off += S * nrb_max * 16 * nt * 4;  // the peers' sums (S - 1 regions) + rank 0's own parked sums
   off = (off + 127) & ~127;
   L.ring = off;
@@ -654,3 +730,23 @@ int launch_decode_mlp_front(const void* x, const void* gqw, const void* gsc, con
 }
 
 }  // namespace b200awq
+
+#ifdef B200AWQ_DECODE_TRACE
+// Trace build only; not part of include/b200awq.h.  Copies up to `cap` records (b200awq::DecTraceRec, 32 bytes each)
+// to host memory `dst`, the kDecMaxSm handoff counters to `pending` (if not null) and returns the number of records
+// written since the last reset (may exceed `cap`); `reset` then empties the buffer.  Synchronises the device.
+extern "C" long long b200awq_decode_trace_read(void* dst, int cap, unsigned int* pending, int reset) {
+  using namespace b200awq;
+  if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+  unsigned int n = 0;
+  if (cudaMemcpyFromSymbol(&n, g_dec_trace_n, sizeof(n)) != cudaSuccess) return -1;
+  const size_t m = std::min<size_t>(std::min<size_t>(n, (size_t)kDecTraceCap), (size_t)std::max(cap, 0));
+  if (m && cudaMemcpyFromSymbol(dst, g_dec_trace, m * sizeof(DecTraceRec)) != cudaSuccess) return -1;
+  if (pending && cudaMemcpyFromSymbol(pending, g_dec_pending, sizeof(g_dec_pending)) != cudaSuccess) return -1;
+  if (reset) {
+    const unsigned int zero = 0;
+    if (cudaMemcpyToSymbol(g_dec_trace_n, &zero, sizeof(zero)) != cudaSuccess) return -1;
+  }
+  return (long long)n;
+}
+#endif
