@@ -44,7 +44,24 @@ std::atomic<bool> g_pdl{true};  // programmatic dependent launch, b200awq_set_pd
 
 bool pdl_enabled() { return g_pdl.load(std::memory_order_relaxed); }
 
-bool aligned16(const void* p) { return p && (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+using b200awq::aligned16;
+
+// `r` passed through; a successful entry that launched a kernel counts one launch (b200awq_launch_count)
+int counted(int r, bool launched) {
+  if (r == 0 && launched) g_launches.fetch_add(1, std::memory_order_relaxed);
+  return r;
+}
+
+// A positive result is the cudaError_t of a launch that could not be configured (e.g. an unschedulable cluster shape):
+// not the caller's problem.  The error is cleared and the result becomes B200AWQ_ERR_SHAPE, so that the next kernel
+// in line gets the shape.
+int next_on_config_error(int r) {
+  if (r <= 0) return r;
+  (void)cudaGetLastError();
+  return B200AWQ_ERR_SHAPE;
+}
+
+int check_dtype(int dtype) { return dtype == B200AWQ_DTYPE_F16 || dtype == B200AWQ_DTYPE_BF16 ? 0 : B200AWQ_ERR_DTYPE; }
 
 int check_device() {
   static std::atomic<signed char> ok[32];  // per device: 0 unknown, 1 ok, -1 wrong device
@@ -62,7 +79,7 @@ int check_device() {
 
 int check_common(const void* x, const void* qw, const void* sc, const void* sz, void* y, int m, int n, int k,
                  int group_size, int dtype) {
-  if (dtype != B200AWQ_DTYPE_F16 && dtype != B200AWQ_DTYPE_BF16) return B200AWQ_ERR_DTYPE;
+  if (int e = check_dtype(dtype)) return e;
   if (group_size != 128) return B200AWQ_ERR_GROUP;
   if (m < 1 || n < 8 || k < 128 || (n % 8) || (k % 128)) return B200AWQ_ERR_SHAPE;
   if (!aligned16(x) || !aligned16(qw) || !aligned16(sc) || !aligned16(sz) || !aligned16(y)) return B200AWQ_ERR_ALIGN;
@@ -90,23 +107,11 @@ bool use_flat(int m, int n, int k) {
 int launch_small(const void* x, const void* qw, const void* sc, const void* sz, void* y, int m, int n, int k, int dtype,
                  cudaStream_t st) {
   int r = B200AWQ_ERR_SHAPE;
-  if (use_decode(m, dtype)) r = b200awq::launch_decode(x, qw, sc, sz, y, n, k, dtype, pdl_enabled(), decode_tuning(), st);
-  if (r > 0) {  // a launch-configuration error (e.g. an unschedulable cluster): the kernels below can take the shape
-    (void)cudaGetLastError();
-    r = B200AWQ_ERR_SHAPE;
-  }
-  if (r != 0 && m <= kRingMaxM) r = b200awq::launch_ring(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st);
-  if (r != 0 && use_flat(m, n, k)) {
-    r = b200awq::launch_flat(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st);
-    if (r > 0) {  // e.g. an unschedulable cluster shape: not the caller's problem, the streaming kernel can take it
-      (void)cudaGetLastError();
-      r = B200AWQ_ERR_SHAPE;
-    }
-  }
-  if (r != 0 && m <= kStreamMaxM) {
-    if (r > 0) (void)cudaGetLastError();
-    r = b200awq::launch_stream(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st);
-  }
+  if (use_decode(m, dtype))
+    r = next_on_config_error(b200awq::launch_decode(x, qw, sc, sz, y, n, k, dtype, pdl_enabled(), decode_tuning(), st));
+  if (r != 0 && m <= kRingMaxM) r = next_on_config_error(b200awq::launch_ring(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st));
+  if (r != 0 && use_flat(m, n, k)) r = next_on_config_error(b200awq::launch_flat(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st));
+  if (r != 0 && m <= kStreamMaxM) r = b200awq::launch_stream(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st);
   return r;
 }
 
@@ -118,9 +123,7 @@ int b200awq_w4a16_gemv(const void* x, const void* qweight, const void* scales, c
                        int k, int group_size, int dtype, void* stream) {
   if (int e = check_common(x, qweight, scales, szeros, y, m, n, k, group_size, dtype)) return e;
   if (m > 7) return B200AWQ_ERR_BATCH;  // reference envelope: gemv_cuda.cu:291-330
-  const int r = launch_small(x, qweight, scales, szeros, y, m, n, k, dtype, static_cast<cudaStream_t>(stream));
-  if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
-  return r;
+  return counted(launch_small(x, qweight, scales, szeros, y, m, n, k, dtype, static_cast<cudaStream_t>(stream)), true);
 }
 
 int b200awq_w4a16_gemv_allreduce(const void* x, const void* qweight, const void* scales, const void* szeros, void* y, int m,
@@ -140,10 +143,9 @@ int b200awq_w4a16_gemv_allreduce(const void* x, const void* qweight, const void*
   pa.world = peers->world;
   pa.tok_cap = peers->cap_words / peers->n_max;
   pa.cap = pa.tok_cap * peers->n_max;
-  int r = b200awq::launch_stream(x, qweight, scales, szeros, y, m, n, k, dtype, pdl_enabled(), static_cast<cudaStream_t>(stream),
-                                 &pa);
-  if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
-  return r;
+  return counted(b200awq::launch_stream(x, qweight, scales, szeros, y, m, n, k, dtype, pdl_enabled(),
+                                        static_cast<cudaStream_t>(stream), &pa),
+                 true);
 }
 
 size_t b200awq_w4a16_mlp_front_workspace_bytes(int m, int n, int) { return m > 0 && n > 0 ? (size_t)2 * m * n * 2 : 0; }
@@ -155,15 +157,11 @@ int b200awq_w4a16_mlp_front(const void* x, const void* gate_qweight, const void*
   if (!aligned16(up_qweight) || !aligned16(up_scales) || !aligned16(up_szeros)) return B200AWQ_ERR_ALIGN;
   if (m >= 8 && n % 128) return B200AWQ_ERR_SHAPE;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (use_decode(m, dtype)) {
-    const int r = b200awq::launch_decode_mlp_front(x, gate_qweight, gate_scales, gate_szeros, up_qweight, up_scales, up_szeros, y,
-                                                   n, k, dtype, pdl_enabled(), decode_tuning(), st);
-    if (r == 0) {
-      g_launches.fetch_add(1, std::memory_order_relaxed);
-      return 0;
-    }
-    if (r > 0) (void)cudaGetLastError();  // launch-configuration error: the composed path below can take the shape
-  }
+  // the fused one-token kernel, else the composed path below: two projections and silu_mul, one count per kernel
+  if (use_decode(m, dtype) &&
+      next_on_config_error(b200awq::launch_decode_mlp_front(x, gate_qweight, gate_scales, gate_szeros, up_qweight, up_scales,
+                                                            up_szeros, y, n, k, dtype, pdl_enabled(), decode_tuning(), st)) == 0)
+    return counted(0, true);
   const size_t half = (size_t)m * n * 2;
   if (!workspace || workspace_bytes < 2 * half || !aligned16(workspace)) return B200AWQ_ERR_WORKSPACE;
   void* g = workspace;
@@ -175,12 +173,9 @@ int b200awq_w4a16_mlp_front(const void* x, const void* gate_qweight, const void*
     int r = B200AWQ_ERR_SHAPE;
     if (m <= 16) r = launch_small(x, qw, sc, sz, t ? u : g, m, n, k, dtype, st);
     if (r == B200AWQ_ERR_SHAPE && n % 128 == 0) r = b200awq::launch_umma(x, qw, sc, sz, t ? u : g, m, n, k, dtype, pdl_enabled(), st);
-    if (r != 0) return r;
-    g_launches.fetch_add(1, std::memory_order_relaxed);
+    if (counted(r, true) != 0) return r;
   }
-  const int r = b200awq::launch_silu_mul(g, u, y, 1, (size_t)m * n, (size_t)m * n, dtype, pdl_enabled(), st);
-  if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
-  return r;
+  return counted(b200awq::launch_silu_mul(g, u, y, 1, (size_t)m * n, (size_t)m * n, dtype, pdl_enabled(), st), true);
 }
 
 size_t b200awq_single_query_attention_workspace_bytes(int batch, int heads, int kv_heads, int head_dim, int max_len) {
@@ -193,23 +188,21 @@ int b200awq_single_query_attention(const void* q, const void* k, const void* v, 
                                    long long v_batch_stride, int rotary_dim, float rotary_base,
                                    float rotary_scale, int neox, int dtype, void* workspace, size_t workspace_bytes,
                                    void* stream) {
-  if (dtype != B200AWQ_DTYPE_F16 && dtype != B200AWQ_DTYPE_BF16) return B200AWQ_ERR_DTYPE;
+  if (int e = check_dtype(dtype)) return e;
   if (!q || !k || !v || !aligned16(k_cache) || !aligned16(v_cache) || !out) return B200AWQ_ERR_ALIGN;
   if (int e = check_device()) return e;
-  const int r = b200awq::launch_single_query_attention(q, k, v, k_cache, v_cache, out, length_per_sample, batch, heads, kv_heads,
-                                                       head_dim, max_len, timestep, q_batch_stride, k_batch_stride, v_batch_stride, rotary_dim,
-                                                       rotary_base,
-                                                       rotary_scale, neox, dtype, workspace, workspace_bytes, pdl_enabled(),
-                                                       static_cast<cudaStream_t>(stream));
-  if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
-  return r;
+  return counted(b200awq::launch_single_query_attention(q, k, v, k_cache, v_cache, out, length_per_sample, batch, heads, kv_heads,
+                                                        head_dim, max_len, timestep, q_batch_stride, k_batch_stride, v_batch_stride,
+                                                        rotary_dim, rotary_base, rotary_scale, neox, dtype, workspace,
+                                                        workspace_bytes, pdl_enabled(), static_cast<cudaStream_t>(stream)),
+                 true);
 }
 
 int b200awq_prefill_attention(const void* q, const void* k, const void* v, void* out, const int* cu_seqlens_q,
                               const int* cu_seqlens_k, int batch, int seqlen_q, int seqlen_k, int heads, int kv_heads,
                               int head_dim, const long long q_strides[3], const long long k_strides[3],
                               const long long v_strides[3], float softmax_scale, int causal, int dtype, void* stream) {
-  if (dtype != B200AWQ_DTYPE_F16 && dtype != B200AWQ_DTYPE_BF16) return B200AWQ_ERR_DTYPE;
+  if (int e = check_dtype(dtype)) return e;
   if (batch < 0 || seqlen_q < 0 || seqlen_k < 0 || heads < 1 || kv_heads < 1 || heads % kv_heads ||
       (head_dim != 64 && head_dim != 72 && head_dim != 128) || !(std::isfinite(softmax_scale) && softmax_scale > 0.f))
     return B200AWQ_ERR_SHAPE;  // the softmax runs on the raw scores' max: scale > 0
@@ -221,11 +214,10 @@ int b200awq_prefill_attention(const void* q, const void* k, const void* v, void*
       if (s[i] % 8) return B200AWQ_ERR_ALIGN;  // TMA takes 16-byte strides
   if (int e = check_device()) return e;
   if (batch == 0 || seqlen_q == 0) return 0;
-  const int r = b200awq::launch_prefill_attention(q, k, v, out, cu_seqlens_q, cu_seqlens_k, batch, seqlen_q, seqlen_k, heads,
-                                                  kv_heads, head_dim, q_strides, k_strides, v_strides, softmax_scale, causal != 0,
-                                                  dtype, static_cast<cudaStream_t>(stream));
-  if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
-  return r;
+  return counted(b200awq::launch_prefill_attention(q, k, v, out, cu_seqlens_q, cu_seqlens_k, batch, seqlen_q, seqlen_k, heads,
+                                                   kv_heads, head_dim, q_strides, k_strides, v_strides, softmax_scale, causal != 0,
+                                                   dtype, static_cast<cudaStream_t>(stream)),
+                 true);
 }
 
 size_t b200awq_splitkv_attention_workspace_bytes(int batch, int seqlen_q, int seqlen_k, int heads, int kv_heads, int head_dim) {
@@ -236,7 +228,7 @@ int b200awq_splitkv_attention(const void* q, const void* k, const void* v, void*
                               int heads, int kv_heads, int head_dim, const long long q_strides[3],
                               const long long k_strides[3], const long long v_strides[3], float softmax_scale, int causal,
                               int dtype, void* workspace, size_t workspace_bytes, void* stream) {
-  if (dtype != B200AWQ_DTYPE_F16 && dtype != B200AWQ_DTYPE_BF16) return B200AWQ_ERR_DTYPE;
+  if (int e = check_dtype(dtype)) return e;
   if (batch < 0 || seqlen_q < 0 || seqlen_k < 0 || heads < 1 || kv_heads < 1 || heads % kv_heads ||
       (long long)seqlen_q * (heads / kv_heads) > 64 || (head_dim != 64 && head_dim != 128) ||
       !(std::isfinite(softmax_scale) && softmax_scale > 0.f))
@@ -252,45 +244,40 @@ int b200awq_splitkv_attention(const void* q, const void* k, const void* v, void*
     return B200AWQ_ERR_WORKSPACE;
   if (int e = check_device()) return e;
   if (batch == 0 || seqlen_q == 0) return 0;
-  const int r = b200awq::launch_splitkv_attention(q, k, v, out, batch, seqlen_q, seqlen_k, heads, kv_heads, head_dim, q_strides,
-                                                  k_strides, v_strides, softmax_scale, causal != 0, dtype, workspace,
-                                                  workspace_bytes, static_cast<cudaStream_t>(stream));
-  if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
-  return r;
+  return counted(b200awq::launch_splitkv_attention(q, k, v, out, batch, seqlen_q, seqlen_k, heads, kv_heads, head_dim, q_strides,
+                                                   k_strides, v_strides, softmax_scale, causal != 0, dtype, workspace,
+                                                   workspace_bytes, static_cast<cudaStream_t>(stream)),
+                 true);
 }
 
 int b200awq_rope_with_pos(const void* x, const float* freqs, void* y, int s, int b, int h, int d, int d2,
                           const long long in_strides[4], const long long out_strides[4], int dtype, void* stream) {
-  if (dtype != B200AWQ_DTYPE_F16 && dtype != B200AWQ_DTYPE_BF16) return B200AWQ_ERR_DTYPE;
+  if (int e = check_dtype(dtype)) return e;
   if (!x || !freqs || !y || !in_strides || !out_strides) return B200AWQ_ERR_ALIGN;
   if (int e = check_device()) return e;
-  const int r = b200awq::launch_rope_with_pos(x, freqs, y, s, b, h, d, d2, in_strides, out_strides, dtype, pdl_enabled(),
-                                              static_cast<cudaStream_t>(stream));
-  if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
-  return r;
+  return counted(b200awq::launch_rope_with_pos(x, freqs, y, s, b, h, d, d2, in_strides, out_strides, dtype, pdl_enabled(),
+                                               static_cast<cudaStream_t>(stream)),
+                 true);
 }
 
 int b200awq_rotary_embedding_neox(const long long* positions, void* query, void* key, const void* cos_sin_cache, int tokens,
                                   int q_heads, int k_heads, int head_size, int rot_dim, long long q_token_stride,
                                   long long k_token_stride, int dtype, void* stream) {
-  if (dtype != B200AWQ_DTYPE_F16 && dtype != B200AWQ_DTYPE_BF16) return B200AWQ_ERR_DTYPE;
+  if (int e = check_dtype(dtype)) return e;
   if (!positions || !cos_sin_cache || (q_heads > 0 && !query) || (k_heads > 0 && !key)) return B200AWQ_ERR_ALIGN;
   if (int e = check_device()) return e;
-  const int r = b200awq::launch_rope_neox(positions, query, key, cos_sin_cache, tokens, q_heads, k_heads, head_size, rot_dim,
-                                          q_token_stride, k_token_stride, dtype, pdl_enabled(), static_cast<cudaStream_t>(stream));
-  if (r == 0 && tokens > 0 && q_heads + k_heads > 0) g_launches.fetch_add(1, std::memory_order_relaxed);
-  return r;
+  return counted(b200awq::launch_rope_neox(positions, query, key, cos_sin_cache, tokens, q_heads, k_heads, head_size, rot_dim,
+                                           q_token_stride, k_token_stride, dtype, pdl_enabled(), static_cast<cudaStream_t>(stream)),
+                 tokens > 0 && q_heads + k_heads > 0);
 }
 
 int b200awq_rmsnorm(const void* x, const void* gamma, void* y, int m, int n, float eps, int dtype, void* stream) {
-  if (dtype != B200AWQ_DTYPE_F16 && dtype != B200AWQ_DTYPE_BF16) return B200AWQ_ERR_DTYPE;
+  if (int e = check_dtype(dtype)) return e;
   if (m < 0 || n < 1) return B200AWQ_ERR_SHAPE;
   if (!x || !gamma || !y) return B200AWQ_ERR_ALIGN;
   if (int e = check_device()) return e;
   if (m == 0) return 0;
-  const int r = b200awq::launch_rmsnorm(x, gamma, y, eps, m, n, dtype, pdl_enabled(), static_cast<cudaStream_t>(stream));
-  if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
-  return r;
+  return counted(b200awq::launch_rmsnorm(x, gamma, y, eps, m, n, dtype, pdl_enabled(), static_cast<cudaStream_t>(stream)), true);
 }
 
 size_t b200awq_w4a16_gemm_workspace_bytes(int, int, int) { return 0; }
@@ -308,8 +295,7 @@ int b200awq_w4a16_gemm(const void* x, const void* qweight, const void* scales, c
   if (m <= 16 && !big_mid) r = launch_small(x, qweight, scales, szeros, y, m, n, k, dtype, static_cast<cudaStream_t>(stream));
   if (r == B200AWQ_ERR_SHAPE)  // 128-channel wgmma tiles; split-k over a cluster for small token counts
     r = b200awq::launch_umma(x, qweight, scales, szeros, y, m, n, k, dtype, pdl_enabled(), static_cast<cudaStream_t>(stream));
-  if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
-  return r;
+  return counted(r, true);
 }
 
 // ---------------------------------------------------------------- W8A8
@@ -320,31 +306,25 @@ int b200awq_w8a8_gemm(const void* x, const void* w, const void* wscales, const v
   if ((reinterpret_cast<uintptr_t>(wscales) | reinterpret_cast<uintptr_t>(ascales) | reinterpret_cast<uintptr_t>(bias)) & 1u)
     return B200AWQ_ERR_ALIGN;
   if (int e = check_device()) return e;
-  const int r = b200awq::launch_w8a8_gemm(x, w, wscales, ascales, bias, y, m, n, k, pdl_enabled(),
-                                          static_cast<cudaStream_t>(stream));
-  if (r == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
-  return r;
+  return counted(b200awq::launch_w8a8_gemm(x, w, wscales, ascales, bias, y, m, n, k, pdl_enabled(), static_cast<cudaStream_t>(stream)),
+                 true);
 }
 
 namespace {
 // common checks of the W8A8 row ops: 16-bit activations, rows the kernels hold in registers, non-null 2-byte aligned
 // pointers (the int8 codes are written one byte at a time when not 16-byte aligned, so any even address will do)
 int check_rows(int m, int n, int dtype, std::initializer_list<const void*> ptrs) {
-  if (dtype != B200AWQ_DTYPE_F16 && dtype != B200AWQ_DTYPE_BF16) return B200AWQ_ERR_DTYPE;
+  if (int e = check_dtype(dtype)) return e;
   if (m < 0 || n < 1 || n > b200awq::w8a8_row_limit()) return B200AWQ_ERR_SHAPE;
   for (const void* p : ptrs)
     if (!p || (reinterpret_cast<uintptr_t>(p) & 1u)) return B200AWQ_ERR_ALIGN;
   return check_device();
 }
-int counted(int r, int m) {
-  if (r == 0 && m > 0) g_launches.fetch_add(1, std::memory_order_relaxed);
-  return r;
-}
 }  // namespace
 
 int b200awq_quant_per_token(const void* x, void* q, void* scales, int m, int n, int dtype, void* stream) {
   if (int e = check_rows(m, n, dtype, {x, scales, q})) return e;
-  return counted(b200awq::launch_quant_per_token(x, q, scales, m, n, dtype, pdl_enabled(), static_cast<cudaStream_t>(stream)), m);
+  return counted(b200awq::launch_quant_per_token(x, q, scales, m, n, dtype, pdl_enabled(), static_cast<cudaStream_t>(stream)), m > 0);
 }
 
 int b200awq_layernorm_quant(const void* x, const void* gamma, const void* beta, void* q, void* scale, int m, int n,
@@ -353,23 +333,23 @@ int b200awq_layernorm_quant(const void* x, const void* gamma, const void* beta, 
   if (int e = check_rows(m, n, dtype, {x, gamma, scale, q})) return e;
   return counted(b200awq::launch_layernorm_quant(x, gamma, beta, q, scale, m, n, eps, per_token != 0, dtype, pdl_enabled(),
                                                  static_cast<cudaStream_t>(stream)),
-                 m);
+                 m > 0);
 }
 
 int b200awq_gelu_quant(const void* x, void* q, void* scales, void* tmp, int m, int n, void* stream) {
   if (int e = check_rows(m, n, B200AWQ_DTYPE_F16, {x, scales, tmp, q})) return e;
-  return counted(b200awq::launch_gelu_quant(x, q, scales, tmp, m, n, pdl_enabled(), static_cast<cudaStream_t>(stream)), m);
+  return counted(b200awq::launch_gelu_quant(x, q, scales, tmp, m, n, pdl_enabled(), static_cast<cudaStream_t>(stream)), m > 0);
 }
 
 int b200awq_silu_and_mul(const void* x, void* y, int m, int d, int dtype, void* stream) {
-  if (dtype != B200AWQ_DTYPE_F16 && dtype != B200AWQ_DTYPE_BF16) return B200AWQ_ERR_DTYPE;
+  if (int e = check_dtype(dtype)) return e;
   if (m < 0 || d < 1) return B200AWQ_ERR_SHAPE;
   if (!x || !y || ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 1u)) return B200AWQ_ERR_ALIGN;
   if (int e = check_device()) return e;
   const char* xb = static_cast<const char*>(x);
   return counted(b200awq::launch_silu_mul(xb, xb + (size_t)d * 2, y, (size_t)m, (size_t)d, (size_t)2 * d, dtype, pdl_enabled(),
                                           static_cast<cudaStream_t>(stream)),
-                 m);
+                 m > 0);
 }
 
 int gemv_forward_4bit(const void* x, const void* qweight, const void* scales, const void* szeros, void* y, int m, int n,

@@ -28,11 +28,6 @@ namespace b200awq {
 namespace {
 
 template <typename T>
-__device__ __forceinline__ float t2f(T v) {
-  if constexpr (TypeTraits<T>::kIsBf16) return __bfloat162float(v);
-  else return __half2float(v);
-}
-template <typename T>
 __device__ __forceinline__ void unpack8(const uint4& v, float (&f)[8]) {
   const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
@@ -161,11 +156,11 @@ __global__ void __launch_bounds__(kAttThreads, 2) single_query_attention_kernel(
       rot = 2 * j < a.rot_dim;
       i0 = 2 * j, i1 = 2 * j + 1;
     }
-    float x = t2f<T>(src[i0]), y = t2f<T>(src[i1]);
+    float x = to_float<T>(src[i0]), y = to_float<T>(src[i1]);
     if (rot) rope_pair(x, y, j, a.rot_dim, tlength, a.base, a.scale);
     const T xr = from_float<T>(x), yr = from_float<T>(y);
     if (g < GS) {
-      qs[g * D + i0] = t2f<T>(xr), qs[g * D + i1] = t2f<T>(yr);
+      qs[g * D + i0] = to_float<T>(xr), qs[g * D + i1] = to_float<T>(yr);
     } else {
       kcur[i0] = xr, kcur[i1] = yr;
       if (writes_cache) {                                  // k -> cache [D / 8][L][8] at slot tlength % L
@@ -331,36 +326,32 @@ __global__ void __launch_bounds__(kAttThreads, 2) single_query_attention_kernel(
   if (tid == 0) a.count[cell] = 0u;  // ready for the next launch (graph replay included)
 }
 
+template <typename T, int GS>
+int launch_att_gs(const AttArgs& a, size_t smem, bool pdl, cudaStream_t stream) {
+  // The size follows the shape (head size, positions per split), so the opt-in is set on every launch that needs it
+  // rather than once per device.
+  if (smem > 48 * 1024) {
+    if (cudaError_t e = cudaFuncSetAttribute(single_query_attention_kernel<T, GS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)smem))
+      return (int)e;
+  }
+  return launch_kernel(single_query_attention_kernel<T, GS>, dim3((unsigned)a.splits, (unsigned)(a.Hkv * a.groups), (unsigned)a.B),
+                       dim3(kAttThreads), smem, stream, pdl, 1, a);
+}
+
 template <typename T>
 int launch_att_g(const AttArgs& a, int GS, size_t smem, bool pdl, cudaStream_t stream) {
-  const void* kern = nullptr;
   switch (GS) {
-    case 1: kern = (const void*)single_query_attention_kernel<T, 1>; break;
-    case 2: kern = (const void*)single_query_attention_kernel<T, 2>; break;
-    case 3: kern = (const void*)single_query_attention_kernel<T, 3>; break;
-    case 4: kern = (const void*)single_query_attention_kernel<T, 4>; break;
-    case 5: kern = (const void*)single_query_attention_kernel<T, 5>; break;
-    case 6: kern = (const void*)single_query_attention_kernel<T, 6>; break;
-    case 7: kern = (const void*)single_query_attention_kernel<T, 7>; break;
-    case 8: kern = (const void*)single_query_attention_kernel<T, 8>; break;
+    case 1: return launch_att_gs<T, 1>(a, smem, pdl, stream);
+    case 2: return launch_att_gs<T, 2>(a, smem, pdl, stream);
+    case 3: return launch_att_gs<T, 3>(a, smem, pdl, stream);
+    case 4: return launch_att_gs<T, 4>(a, smem, pdl, stream);
+    case 5: return launch_att_gs<T, 5>(a, smem, pdl, stream);
+    case 6: return launch_att_gs<T, 6>(a, smem, pdl, stream);
+    case 7: return launch_att_gs<T, 7>(a, smem, pdl, stream);
+    case 8: return launch_att_gs<T, 8>(a, smem, pdl, stream);
     default: return B200AWQ_ERR_SHAPE;
   }
-  if (smem > 48 * 1024) {
-    if (cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) return (int)e;
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)a.splits, (unsigned)(a.Hkv * a.groups), (unsigned)a.B);
-  cfg.blockDim = dim3(kAttThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
-  void* args[] = {const_cast<AttArgs*>(&a)};
-  cudaError_t e = cudaLaunchKernelExC(&cfg, kern, args);
-  return e == cudaSuccess ? 0 : (int)e;
 }
 
 // ------------------------------------------------------------------------------------------------ RoPE over [s, b, h, d]
@@ -383,11 +374,11 @@ __global__ void __launch_bounds__(256) rope_with_pos_kernel(const RopeArgs a) {
   for (int i = threadIdx.x; i < a.h * a.d; i += blockDim.x) {
     const int h_id = i / a.d, d_id = i % a.d;
     const T* sp = src + h_id * a.sh;
-    float v = t2f<T>(sp[d_id * a.sd]);
+    float v = to_float<T>(sp[d_id * a.sd]);
     if (d_id < a.d2) {
       float sn, cs;
       sincosf(fr[d_id], &sn, &cs);
-      const float rot = (d_id + a.d2 / 2 < a.d2) ? -t2f<T>(sp[(d_id + a.d2 / 2) * a.sd]) : t2f<T>(sp[(d_id - a.d2 / 2) * a.sd]);
+      const float rot = (d_id + a.d2 / 2 < a.d2) ? -to_float<T>(sp[(d_id + a.d2 / 2) * a.sd]) : to_float<T>(sp[(d_id - a.d2 / 2) * a.sd]);
       v = v * cs + rot * sn;  // fused_rope_with_pos.cu:52-57
     }
     dst[h_id * a.oh + d_id * a.od] = from_float<T>(v);
@@ -428,8 +419,8 @@ int launch_single_query_attention(const void* q, const void* k, const void* v, v
   a.inv_sqrt_d = 1.f / sqrtf((float)head_dim);
   // worst-case positions (length_per_sample is on the device): the chunking must cover up to min(timestep, max_len - 1) + 1
   const int npos_max = std::min(length_per_sample ? max_len : timestep + 1, max_len);
-  int dev = 0, nsm = 132;
-  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+  const int nsm = sm_count();
+  if (nsm == 0) return B200AWQ_ERR_DEVICE;
   const int chunk_cap = std::max(256, (48 * 1024 / 4) / GS / 32 * 32);  // logits of a chunk: GS * chunk floats <= 48 KB
   int splits = std::max(1, std::min(64, 2 * nsm / std::max(1, batch * kv_heads * groups)));
   splits = std::min(splits, (npos_max + 127) / 128);                  // >= 128 positions per CTA
@@ -453,19 +444,9 @@ int launch_rope_with_pos(const void* x, const float* freqs, void* y, int s, int 
   if (s < 1 || b < 1 || h < 1 || d < 1 || d2 < 0 || d2 > d || (d2 & 1)) return B200AWQ_ERR_SHAPE;
   RopeArgs a{x, freqs, y, s, b, h, d, d2, in_strides[0], in_strides[1], in_strides[2], in_strides[3],
              out_strides[0], out_strides[1], out_strides[2], out_strides[3]};
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)s, (unsigned)b);
-  cfg.blockDim = dim3(256);
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
-  cudaError_t e;
-  if (dtype == B200AWQ_DTYPE_F16) e = cudaLaunchKernelEx(&cfg, rope_with_pos_kernel<__half>, a);
-  else e = cudaLaunchKernelEx(&cfg, rope_with_pos_kernel<__nv_bfloat16>, a);
-  return e == cudaSuccess ? 0 : (int)e;
+  const dim3 grid((unsigned)s, (unsigned)b);
+  if (dtype == B200AWQ_DTYPE_F16) return launch_kernel(rope_with_pos_kernel<__half>, grid, dim3(256), 0, stream, pdl, 1, a);
+  return launch_kernel(rope_with_pos_kernel<__nv_bfloat16>, grid, dim3(256), 0, stream, pdl, 1, a);
 }
 
 }  // namespace b200awq

@@ -7,12 +7,6 @@
 
 namespace b200awq {
 
-template <int NA>
-__device__ __forceinline__ void acc_fence(float (&d)[NA]) {
-#pragma unroll
-  for (int i = 0; i < NA; ++i) asm volatile("" : "+f"(d[i])::"memory");
-}
-
 // S[64 x 128] (+)= A[64 x 16] * B[16 x 128], both operands K-major in shared memory (Q rows, K rows), fp32 accumulate
 #define B200AWQ_WGMMA_SS_N128(TY)                                                                                            \
   asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"                                                                \

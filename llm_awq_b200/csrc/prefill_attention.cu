@@ -330,15 +330,13 @@ int launch_t(const void* q, const void* k, const void* v, void* out, const int* 
     if (int e = encode_bthd<T>(enc, &tm[4], k, head_dim, tk, kv_heads, nb, ks, 16, kBN)) return e;
     if (int e = encode_bthd<T>(enc, &tm[5], v, head_dim, tk, kv_heads, nb, vs, 16, kBN)) return e;
   }
-  auto kern = prefill_attention_kernel<T, DP>;
-  static bool attr_set[32] = {};  // per instantiation and device
-  if (cudaError_t ea = ensure_dyn_smem(kern, C::kSmem, attr_set)) return (int)ea;
+  if (cudaError_t ea = ensure_dyn_smem<prefill_attention_kernel<T, DP>>(C::kSmem)) return (int)ea;
   const dim3 grid((unsigned)heads, (unsigned)batch, (unsigned)((seqlen_q + kBM - 1) / kBM));
   const float scale_log2 = softmax_scale * 1.4426950408889634f;
-  kern<<<grid, kThreads, C::kSmem, stream>>>(tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], static_cast<T*>(out), cu_q, cu_k, seqlen_q, seqlen_k, heads,
-                                             heads / kv_heads, head_dim, scale_log2, causal ? 1 : 0);
-  const cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : (int)e;
+  // no programmatic dependent launch: the kernel never waits on the previous grid
+  return launch_kernel(prefill_attention_kernel<T, DP>, grid, dim3(kThreads), (size_t)C::kSmem, stream, false, 1, tm[0], tm[1],
+                       tm[2], tm[3], tm[4], tm[5], out, cu_q, cu_k, seqlen_q, seqlen_k, heads, heads / kv_heads, head_dim,
+                       scale_log2, causal ? 1 : 0);
 }
 
 template <typename T>

@@ -26,11 +26,6 @@ __device__ __forceinline__ float2 pair_to_float2(uint32_t v) {
   if constexpr (TypeTraits<T>::kIsBf16) return __bfloat1622float2(u32_as_b2(v));
   else return __half22float2(u32_as_h2(v));
 }
-template <typename T>
-__device__ __forceinline__ float elem_to_float(T v) {
-  if constexpr (TypeTraits<T>::kIsBf16) return __bfloat162float(v);
-  else return __half2float(v);
-}
 // reduction.cuh:72-82: finite clamp for fp16 only
 template <typename T>
 __device__ __forceinline__ T norm_round(float v) {
@@ -117,39 +112,26 @@ __global__ void __launch_bounds__(kNormThreads) rmsnorm_generic_kernel(const T* 
   for (int c = threadIdx.x; c < (n + 7) / 8; c += kNormThreads) {
     const int end = min(8 * c + 8, n);
     for (int i = 8 * c; i < end; ++i) {
-      const float f = elem_to_float<T>(xr[i]);
+      const float f = to_float<T>(xr[i]);
       s = fmaf(f, f, s);
     }
   }
   const float r = rsqrtf(block_sum(s, red) / (float)n + eps);
   T* yr = y + (size_t)blockIdx.x * n;
   for (int i = threadIdx.x; i < n; i += kNormThreads)
-    yr[i] = norm_round<T>((elem_to_float<T>(xr[i]) * r) * elem_to_float<T>(gamma[i]));
+    yr[i] = norm_round<T>((to_float<T>(xr[i]) * r) * to_float<T>(gamma[i]));
 }
 
 template <typename T>
 int launch_t(const void* x, const void* gamma, void* y, float eps, int m, int n, bool pdl, cudaStream_t stream) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)m);
-  cfg.blockDim = dim3(kNormThreads);
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
-  const T* xp = static_cast<const T*>(x);
-  const T* gp = static_cast<const T*>(gamma);
-  T* yp = static_cast<T*>(y);
-  const bool vec = n % 8 == 0 && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(y)) & 15u) == 0;
+  const bool vec = n % 8 == 0 && aligned16(x) && aligned16(gamma) && aligned16(y);
   const int per = (n / 8 + kNormThreads - 1) / kNormThreads;
-  cudaError_t e;
-  if (vec && per <= 1) e = cudaLaunchKernelEx(&cfg, rmsnorm_rows_kernel<T, 1>, xp, gp, yp, eps, n);
-  else if (vec && per <= 2) e = cudaLaunchKernelEx(&cfg, rmsnorm_rows_kernel<T, 2>, xp, gp, yp, eps, n);
-  else if (vec && per <= 4) e = cudaLaunchKernelEx(&cfg, rmsnorm_rows_kernel<T, 4>, xp, gp, yp, eps, n);
-  else if (vec && per <= 8) e = cudaLaunchKernelEx(&cfg, rmsnorm_rows_kernel<T, 8>, xp, gp, yp, eps, n);
-  else e = cudaLaunchKernelEx(&cfg, rmsnorm_generic_kernel<T>, xp, gp, yp, eps, n);
-  return e == cudaSuccess ? 0 : (int)e;
+  const dim3 grid((unsigned)m), block(kNormThreads);
+  if (vec && per <= 1) return launch_kernel(rmsnorm_rows_kernel<T, 1>, grid, block, 0, stream, pdl, 1, x, gamma, y, eps, n);
+  if (vec && per <= 2) return launch_kernel(rmsnorm_rows_kernel<T, 2>, grid, block, 0, stream, pdl, 1, x, gamma, y, eps, n);
+  if (vec && per <= 4) return launch_kernel(rmsnorm_rows_kernel<T, 4>, grid, block, 0, stream, pdl, 1, x, gamma, y, eps, n);
+  if (vec && per <= 8) return launch_kernel(rmsnorm_rows_kernel<T, 8>, grid, block, 0, stream, pdl, 1, x, gamma, y, eps, n);
+  return launch_kernel(rmsnorm_generic_kernel<T>, grid, block, 0, stream, pdl, 1, x, gamma, y, eps, n);
 }
 
 }  // namespace

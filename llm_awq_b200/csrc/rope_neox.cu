@@ -23,17 +23,10 @@ template <typename T>
 static int launch_neox_t(const RopeNeoxArgs& a, bool pdl, cudaStream_t stream) {
   const bool vec = rope_neox_can_vectorise(a);
   const int items = vec ? rope_neox_items<8>(a) : rope_neox_items<1>(a);
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)std::min(a.tokens, 65535 * 8));
-  cfg.blockDim = dim3((unsigned)std::min(512, std::max(32, (items + 31) / 32 * 32)));
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
-  const cudaError_t e = vec ? cudaLaunchKernelEx(&cfg, rope_neox_kernel<T, 8>, a) : cudaLaunchKernelEx(&cfg, rope_neox_kernel<T, 1>, a);
-  return e == cudaSuccess ? 0 : (int)e;
+  const dim3 grid((unsigned)std::min(a.tokens, 65535 * 8));
+  const dim3 block((unsigned)std::min(512, std::max(32, (items + 31) / 32 * 32)));
+  if (vec) return launch_kernel(rope_neox_kernel<T, 8>, grid, block, 0, stream, pdl, 1, a);
+  return launch_kernel(rope_neox_kernel<T, 1>, grid, block, 0, stream, pdl, 1, a);
 }
 
 int launch_rope_neox(const long long* positions, void* query, void* key, const void* cos_sin, int tokens, int q_heads,

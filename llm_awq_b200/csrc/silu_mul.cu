@@ -51,29 +51,16 @@ int launch_silu_mul(const void* gate, const void* up, void* out, size_t rows, si
                     cudaStream_t stream) {
   const size_t count = rows * cols;
   if (count == 0) return 0;
-  auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
   // 16-byte accesses need every row start aligned (a single row only needs the base pointers aligned)
-  const bool vec = a16(gate) && a16(up) && a16(out) && (rows == 1 || (cols % 8 == 0 && in_pitch % 8 == 0));
-  int dev = 0, nsm = 132;
-  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+  const bool vec = aligned16(gate) && aligned16(up) && aligned16(out) && (rows == 1 || (cols % 8 == 0 && in_pitch % 8 == 0));
+  const int nsm = sm_count();
+  if (nsm == 0) return B200AWQ_ERR_DEVICE;
   const size_t want = ((vec ? count / 8 : count) + 255) / 256;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)std::max<size_t>(1, std::min<size_t>(want, (size_t)nsm * 8)));
-  cfg.blockDim = dim3(256);
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
-  cudaError_t e;
+  const dim3 grid((unsigned)std::max<size_t>(1, std::min<size_t>(want, (size_t)nsm * 8)));
   if (dtype == B200AWQ_DTYPE_F16)
-    e = cudaLaunchKernelEx(&cfg, silu_mul_kernel<__half>, static_cast<const __half*>(gate), static_cast<const __half*>(up),
-                           static_cast<__half*>(out), rows, cols, in_pitch, vec);
-  else
-    e = cudaLaunchKernelEx(&cfg, silu_mul_kernel<__nv_bfloat16>, static_cast<const __nv_bfloat16*>(gate),
-                           static_cast<const __nv_bfloat16*>(up), static_cast<__nv_bfloat16*>(out), rows, cols, in_pitch, vec);
-  return e == cudaSuccess ? 0 : (int)e;
+    return launch_kernel(silu_mul_kernel<__half>, grid, dim3(256), 0, stream, pdl, 1, gate, up, out, rows, cols, in_pitch, vec);
+  return launch_kernel(silu_mul_kernel<__nv_bfloat16>, grid, dim3(256), 0, stream, pdl, 1, gate, up, out, rows, cols, in_pitch,
+                       vec);
 }
 
 }  // namespace b200awq

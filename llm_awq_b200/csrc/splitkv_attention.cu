@@ -347,9 +347,8 @@ int launch_t(const void* q, const void* k, const void* v, void* out, int batch, 
              int kv_heads, const long long* qs, const long long* ks, const long long* vs, float softmax_scale, bool causal,
              void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   using C = SplitCfg<D>;
-  int dev = 0, sms = 132;
-  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  sms = std::max(1, std::min(sms, kMaxSms));
+  const int sms = std::min(sm_count(), kMaxSms);
+  if (sms == 0) return B200AWQ_ERR_DEVICE;
   SplitArgs a{};
   a.q = q, a.out = out;
   a.qs0 = qs[0], a.qs1 = qs[1], a.qs2 = qs[2];
@@ -370,13 +369,10 @@ int launch_t(const void* q, const void* k, const void* v, void* out, int batch, 
   CUtensorMap tm[2];
   if (int e = encode_bthd<T>(enc, &tm[0], k, D, seqlen_k, kv_heads, batch, ks, 64, kBN)) return e;
   if (int e = encode_bthd<T>(enc, &tm[1], v, D, seqlen_k, kv_heads, batch, vs, 64, kBN)) return e;
-  auto kern = splitkv_attention_kernel<T, D>;
-  static bool attr_set[32] = {};  // per instantiation and device
-  if (cudaError_t ea = ensure_dyn_smem(kern, C::kSmem, attr_set)) return (int)ea;
-  const dim3 grid((unsigned)a.splits, (unsigned)kv_heads, (unsigned)batch);
-  kern<<<grid, kThreads, C::kSmem, stream>>>(tm[0], tm[1], a);
-  const cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : (int)e;
+  if (cudaError_t ea = ensure_dyn_smem<splitkv_attention_kernel<T, D>>(C::kSmem)) return (int)ea;
+  // no programmatic dependent launch: the kernel never waits on the previous grid
+  return launch_kernel(splitkv_attention_kernel<T, D>, dim3((unsigned)a.splits, (unsigned)kv_heads, (unsigned)batch),
+                       dim3(kThreads), (size_t)C::kSmem, stream, false, 1, tm[0], tm[1], a);
 }
 
 template <typename T>

@@ -1,5 +1,6 @@
-// Shared device helpers for the sm_90a W4A16 kernels: packed-format index math,
-// exact int4 -> fp16/bf16 dequantisation, mbarrier / bulk-copy / PDL / cluster PTX.
+// Shared device helpers for the sm_90a kernels: packed-format index math, exact int4 -> fp16/bf16
+// dequantisation, and one copy of every PTX wrapper more than one kernel uses (shared-memory loads,
+// cp.async, mbarrier, bulk copy, PDL, cluster, wgmma accumulator fences).
 //
 // Packed format (closed form of the reference packer awq/quantize/qmodule.py:26-65):
 // qweight is int16 [N/4, K].  Each 4-row x 64-k tile is one contiguous 128-byte segment
@@ -108,9 +109,61 @@ __device__ __forceinline__ T from_float(float v);
 template <> __device__ __forceinline__ __half from_float<__half>(float v) { return __float2half_rn(v); }
 template <> __device__ __forceinline__ __nv_bfloat16 from_float<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
 
-// ---------------------------------------------------------------- shared-memory addresses
+template <typename T>
+__device__ __forceinline__ float to_float(T v);
+template <> __device__ __forceinline__ float to_float<__half>(__half v) { return __half2float(v); }
+template <> __device__ __forceinline__ float to_float<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
+
+// keeps the compiler from moving accumulator reads / writes across a wgmma fence or wait
+template <int NA>
+__device__ __forceinline__ void acc_fence(float (&d)[NA]) {
+#pragma unroll
+  for (int i = 0; i < NA; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+template <int NA>
+__device__ __forceinline__ void acc_fence(int (&d)[NA]) {
+#pragma unroll
+  for (int i = 0; i < NA; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
+
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+
+// ---------------------------------------------------------------- shared memory
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
+}
+__device__ __forceinline__ void ldsm4(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr));
+}
+__device__ __forceinline__ uint4 lds128(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ uint16_t lds16(uint32_t addr) {
+  uint16_t v;
+  asm volatile("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(addr));
+  return v;
+}
+
+// ---------------------------------------------------------------- cp.async (8 or 16 bytes, global -> shared)
+template <int kBytes>
+__device__ __forceinline__ void cp_async(uint32_t dst, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], %2;" ::"r"(dst), "l"(src), "n"(kBytes) : "memory");
+}
+template <int kBytes>
+__device__ __forceinline__ void cp_async(void* dst, const void* src) {
+  cp_async<kBytes>(smem_u32(dst), src);
+}
+// arrival on `bar` once this thread's earlier cp.async copies have landed (does not count as an expected arrival)
+__device__ __forceinline__ void cp_async_mbar_arrive(uint64_t* bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
 // ---------------------------------------------------------------- mbarrier
@@ -183,6 +236,8 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
 // address of `local_smem_addr` in CTA `rank` of the cluster (shared::cluster window)
 __device__ __forceinline__ uint32_t map_to_rank(uint32_t local_smem_addr, uint32_t rank) {
   uint32_t a;
@@ -194,12 +249,17 @@ __device__ __forceinline__ float ld_cluster_f32(uint32_t cluster_addr) {
   asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(cluster_addr) : "memory");
   return v;
 }
+// one fp32 into a peer CTA's shared memory (`cluster_addr`), completing 4 bytes on its mbarrier at `cluster_bar`
+__device__ __forceinline__ void st_async_f32(uint32_t cluster_addr, float v, uint32_t cluster_bar) {
+  asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(cluster_addr),
+               "r"(__float_as_uint(v)), "r"(cluster_bar)
+               : "memory");
+}
 
 // ---------------------------------------------------------------- warp-level tensor-core MAC
 // D[16 x 8] = A[16 x 16] * B[16 x 8] + C, fp32 accumulate.  Not `volatile`: a pure function of its register
-// operands, so the compiler may interleave independent groups.  Used by the HBM-bound streaming
-// kernel only: rows of A are output channels (dequantised in registers), columns of B are
-// tokens.
+// operands, so the compiler may interleave independent groups.  Used by the HBM-bound streaming and ring
+// kernels: rows of A are output channels (dequantised in registers), columns of B are tokens.
 template <typename T>
 __device__ __forceinline__ void mma_16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
                                           uint32_t b0, uint32_t b1, const float (&c)[4]) {

@@ -85,8 +85,8 @@ constexpr int kDecTraceCap = 1 << 20;
 __device__ DecTraceRec g_dec_trace[kDecTraceCap];
 __device__ unsigned int g_dec_trace_n;
 __device__ __forceinline__ void dec_trace(const void* layer, int event) {
-  unsigned long long t, c;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  unsigned long long c;
+  const unsigned long long t = globaltimer_ns();
   asm volatile("mov.u64 %0, %%clock64;" : "=l"(c));
   if (threadIdx.x & 31) return;  // one record per warp
   const unsigned int i = atomicAdd(&g_dec_trace_n, 1u);
@@ -118,32 +118,9 @@ struct DecArgs {
   DecLayout L;
 };
 
-__device__ __forceinline__ void dec_cp_async8(uint32_t dst, const void* src) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(dst), "l"(src) : "memory");
-}
-__device__ __forceinline__ void dec_cp_async_arrive(uint64_t* bar) {
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void dec_ldsm4(uint32_t (&r)[4], uint32_t addr) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(addr));
-}
-__device__ __forceinline__ uint4 dec_lds128(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ uint16_t dec_lds16(uint32_t addr) {
-  uint16_t v;
-  asm volatile("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(addr));
-  return v;
-}
 __device__ __forceinline__ void dec_sts8(uint32_t addr, int v) {
   asm volatile("st.shared.u8 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
-__device__ __forceinline__ void dec_cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
-__device__ __forceinline__ void dec_cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
 __device__ __forceinline__ void dec_imma(int (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1,
                                          const int (&c)[4]) {
   asm("mma.sync.aligned.m16n8k32.row.col.s32.u8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%10,%11,%12,%13};"
@@ -270,7 +247,7 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
           if (use > 0 || slot == hold) {
             if (!joined) {
               asm volatile("bar.sync 0;" ::: "memory");  // the CTA barrier the other warps wait at (below)
-              if (S > 1) dec_cluster_arrive();
+              if (S > 1) cluster_arrive();
               joined = true;
               DEC_TRACE(a.qw, kTrFirstLap);
             }
@@ -302,14 +279,14 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
           if (lane < ng) {  // lane = group: 8 bytes (4 channels) of scales and of zeros per quad row
             const size_t off = ((size_t)(g0 + lane) * N + (size_t)q0 * 4) * 2;
             const uint32_t dst = smem_u32(sw) + kDecScaleOff + lane * 8;
-            dec_cp_async8(dst, sct + off);
-            dec_cp_async8(dst + kDecPiece * 8, szt + off);
+            cp_async<8>(dst, sct + off);
+            cp_async<8>(dst + kDecPiece * 8, szt + off);
             if (nqs > 1) {
-              dec_cp_async8(dst + 2 * kDecPiece * 8, sct + off + 8);
-              dec_cp_async8(dst + 3 * kDecPiece * 8, szt + off + 8);
+              cp_async<8>(dst + 2 * kDecPiece * 8, sct + off + 8);
+              cp_async<8>(dst + 3 * kDecPiece * 8, szt + off + 8);
             }
           }
-          dec_cp_async_arrive(&full[slot]);
+          cp_async_mbar_arrive(&full[slot]);
           if (++slot == NS) slot = 0, ++use;
         }
       }
@@ -319,15 +296,15 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
     DEC_TRACE(a.qw, kTrLastIssue);
     if (!joined) {
       asm volatile("bar.sync 0;" ::: "memory");
-      if (S > 1) dec_cluster_arrive();
+      if (S > 1) cluster_arrive();
     }
-    if (S > 1) dec_cluster_wait();
+    if (S > 1) cluster_wait();
     return;
   }
 
   asm volatile("bar.sync 0;" ::: "memory");  // barrier inits of both initialising warps are visible (the producer joins after its first lap)
-  if (S > 1) dec_cluster_arrive();  // publishes rank 0's exchange barriers to the peers
-  if (S > 1) dec_cluster_wait();
+  if (S > 1) cluster_arrive();  // publishes rank 0's exchange barriers to the peers
+  if (S > 1) cluster_wait();
   // Consumers: everything the first activation loads need is computed BEFORE the dependency wait, and the loads are the
   // first instructions after it (measured: ~470 cycles passed between the wait returning and the loads issuing when the
   // address arithmetic -- kernel parameters from the constant bank, cold instructions -- came after the wait).
@@ -389,10 +366,7 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
       } else if (rank > 0) {
         if (mine && ch < nch) {
           const uint32_t dbar = map_to_rank(smem_u32(&xch[rb]), 0);
-          const uint32_t dst = map_to_rank(smem_u32(&xchg[((rank - 1) * a.nrb_max + rb) * RW + lane]), 0);
-          asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(dst),
-                       "r"(__float_as_uint(v)), "r"(dbar)
-                       : "memory");
+          st_async_f32(map_to_rank(smem_u32(&xchg[((rank - 1) * a.nrb_max + rb) * RW + lane]), 0), v, dbar);
         }
       } else {
         if (mine) hold[rb * RW + lane] = v;  // read back by the same lane only
@@ -547,12 +521,12 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
       const uint32_t cA_item = sa_u32 + sc_off + coef_sel, cB_item = sb_u32 + sc_off + coef_sel;
       auto mac_group = [&](const uint32_t gi) {
         uint32_t w0[4], w1[4];
-        dec_ldsm4(w0, w_lane + gi * 256u);
-        dec_ldsm4(w1, w_lane + gi * 256u + 128u);
-        const uint4 bv = dec_lds128(xd_item + gi * (uint32_t)kDecGroupBytes);
+        ldsm4(w0, w_lane + gi * 256u);
+        ldsm4(w1, w_lane + gi * 256u + 128u);
+        const uint4 bv = lds128(xd_item + gi * (uint32_t)kDecGroupBytes);
         float gv;
         asm volatile("ld.shared.f32 %0, [%1];" : "=f"(gv) : "r"(gx_item + gi * 16u));
-        const uint16_t cA = dec_lds16(cA_item + gi * 8u), cB = dec_lds16(cB_item + gi * 8u);
+        const uint16_t cA = lds16(cA_item + gi * 8u), cB = lds16(cB_item + gi * 8u);
         int accR[4], accH[4];
         dec_imma(accR, w0[0], w0[1], w0[2], w0[3], bv.x, bv.y, zero4);
         dec_imma(accH, w0[0] & 0xf0f0f0f0u, w0[1] & 0xf0f0f0f0u, w0[2] & 0xf0f0f0f0u, w0[3] & 0xf0f0f0f0u, bv.x, bv.y, zero4);
@@ -610,30 +584,13 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
 
 // ------------------------------------------------------------------------------------ host
 namespace {
-
-int dec_sm_count() {
-  static int cnt[32] = {};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
-  dev &= 31;
-  if (cnt[dev] == 0) {
-    int v = 0;
-    cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    cnt[dev] = v;
-  }
-  return cnt[dev];
-}
-
-}  // namespace
-
-namespace {
 int launch_decode_impl(const void* x, const void* qw, const void* sc, const void* sz, const void* qw2, const void* sc2,
                        const void* sz2, void* y, int N, int K, int dtype, bool pdl, const DecodeTuning& tune, cudaStream_t stream) {
   const bool fused = qw2 != nullptr;
   const int nt = fused ? 2 : 1;
   if (dtype != B200AWQ_DTYPE_F16 || N % 8 || K % kGroup) return B200AWQ_ERR_SHAPE;
-  const int nsm = dec_sm_count();
-  if (nsm < 1) return B200AWQ_ERR_SHAPE;
+  const int nsm = sm_count();
+  if (nsm == 0) return B200AWQ_ERR_DEVICE;
   const int G = K / kGroup, Q = N / 4;
   DecArgs a{};
   a.x = x, a.qw = static_cast<const uint16_t*>(qw), a.sc = sc, a.sz = sz, a.y = y;
@@ -681,39 +638,13 @@ int launch_decode_impl(const void* x, const void* qw, const void* sc, const void
   a.NS = ns;
   L.total = off + ns * kDecSlotBytes;
 
-  static bool attr_set[2][32] = {};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return B200AWQ_ERR_DEVICE;
-  const void* kern = fused ? (const void*)w4a16_decode_kernel<true> : (const void*)w4a16_decode_kernel<false>;
-  if (!attr_set[fused][dev & 31]) {
-    if (cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemBudget)) return (int)e;
-    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    attr_set[fused][dev & 31] = true;
+  const dim3 grid((unsigned)(a.units * a.S)), block((unsigned)((kDecCons + 2) * 32));
+  if (fused) {
+    if (cudaError_t e = ensure_dyn_smem<w4a16_decode_kernel<true>>(kDecSmemBudget, true)) return (int)e;
+    return launch_kernel(w4a16_decode_kernel<true>, grid, block, (size_t)L.total, stream, pdl, (unsigned)a.S, a);
   }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(a.units * a.S));
-  cfg.blockDim = dim3((unsigned)((kDecCons + 2) * 32));
-  cfg.dynamicSmemBytes = (size_t)L.total;
-  cfg.stream = stream;
-  cudaLaunchAttribute attrs[2];
-  int na = 0;
-  if (a.S > 1) {
-    attrs[na].id = cudaLaunchAttributeClusterDimension;
-    attrs[na].val.clusterDim.x = (unsigned)a.S;
-    attrs[na].val.clusterDim.y = 1;
-    attrs[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  if (pdl) {
-    attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attrs[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  cfg.attrs = attrs;
-  cfg.numAttrs = na;
-  void* args[] = {const_cast<DecArgs*>(&a)};
-  cudaError_t e = cudaLaunchKernelExC(&cfg, kern, args);
-  return e == cudaSuccess ? 0 : (int)e;
+  if (cudaError_t e = ensure_dyn_smem<w4a16_decode_kernel<false>>(kDecSmemBudget, true)) return (int)e;
+  return launch_kernel(w4a16_decode_kernel<false>, grid, block, (size_t)L.total, stream, pdl, (unsigned)a.S, a);
 }
 }  // namespace
 

@@ -1,24 +1,76 @@
-// Internal launcher interface between the C ABI (api.cu) and the kernel translation units.
+// Internal launcher interface between the C ABI (api.cu) and the kernel translation units, and the host launch path
+// every launcher shares.
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
+#include <stdint.h>
+
+#include <atomic>
 
 #include "../../include/b200awq.h"
 
 namespace b200awq {
 
-// Opt a kernel into a large dynamic shared-memory size once PER DEVICE (several GPUs may be driven from one process;
-// function attributes are per device).  `flags` is a function-local static array of the caller.
-template <typename K>
-inline cudaError_t ensure_dyn_smem(K kern, int bytes, bool (&flags)[32]) {
+inline bool aligned16(const void* p) { return p && (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+// Per-device host caches hold this many devices; a device with a higher ordinal is served uncached.
+constexpr int kMaxCachedDevices = 64;
+
+// The current device's SM count, cached per device; 0 if the query fails.
+inline int sm_count() {
+  static std::atomic<int> cache[kMaxCachedDevices];
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
+  if (dev < kMaxCachedDevices && (n = cache[dev].load(std::memory_order_relaxed)) > 0) return n;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 0) return 0;
+  if (dev < kMaxCachedDevices) cache[dev].store(n, std::memory_order_relaxed);
+  return n;
+}
+
+// Opt kernel `Kern` into `bytes` of dynamic shared memory once per device (function attributes are per device, and
+// several GPUs may be driven from one process); `max_shared_carveout` also asks for the largest shared-memory carveout.
+template <auto Kern>
+inline cudaError_t ensure_dyn_smem(int bytes, bool max_shared_carveout = false) {
+  static std::atomic<bool> done[kMaxCachedDevices];
   int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  dev &= 31;
-  if (flags[dev]) return cudaSuccess;
-  e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e == cudaSuccess) flags[dev] = true;
-  return e;
+  if (cudaError_t e = cudaGetDevice(&dev)) return e;
+  const bool cached = dev < kMaxCachedDevices;
+  if (cached && done[dev].load(std::memory_order_acquire)) return cudaSuccess;
+  if (cudaError_t e = cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)) return e;
+  if (max_shared_carveout)
+    cudaFuncSetAttribute(Kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  if (cached) done[dev].store(true, std::memory_order_release);
+  return cudaSuccess;
+}
+
+// Launches `kern` with programmatic dependent launch when `pdl` and in clusters of `cluster_x` CTAs when > 1.
+// Returns 0 or the launch's cudaError_t.
+template <typename... KArgs, typename... Args>
+int launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, bool pdl,
+                  unsigned cluster_x, Args... args) {
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attrs[2];
+  int na = 0;
+  if (cluster_x > 1) {
+    attrs[na].id = cudaLaunchAttributeClusterDimension;
+    attrs[na].val.clusterDim.x = cluster_x;
+    attrs[na].val.clusterDim.y = 1;
+    attrs[na].val.clusterDim.z = 1;
+    ++na;
+  }
+  if (pdl) {
+    attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attrs[na].val.programmaticStreamSerializationAllowed = 1;
+    ++na;
+  }
+  cfg.attrs = attrs;
+  cfg.numAttrs = na;
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
+  return e == cudaSuccess ? 0 : (int)e;
 }
 
 // Every launcher below picks its kernel configuration (instantiation, k split, grid, ring depth, shared-memory size)
@@ -43,7 +95,7 @@ int launch_stream(const void* x, const void* qw, const void* sc, const void* sz,
 int launch_umma(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
                 bool pdl, cudaStream_t stream);
 
-// persistent warp-specialised decode kernel, 1 <= M <= 8 (w4a16_ring.cu); returns B200AWQ_ERR_SHAPE when the
+// persistent warp-specialised decode kernel, 1 <= M <= 4 (w4a16_ring.cu); returns B200AWQ_ERR_SHAPE when the
 // activations do not fit next to a useful ring (the caller falls back to the kernels below)
 int launch_ring(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
                 bool pdl, cudaStream_t stream);
@@ -102,7 +154,7 @@ int launch_splitkv_attention(const void* q, const void* k, const void* v, void* 
                              const long long* v_strides, float softmax_scale, bool causal, int dtype, void* workspace,
                              size_t workspace_bytes, cudaStream_t stream);
 
-// the same kernel for skinny batches, 1 <= M <= 64, N % 128 == 0: one CTA per tile and k slice (w4a16_wgmma.cu)
+// the same kernel for skinny batches, 1 <= M <= 16, N % 128 == 0: one CTA per tile and k slice (w4a16_wgmma.cu)
 int launch_flat(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
                 bool pdl, cudaStream_t stream);
 

@@ -1,4 +1,4 @@
-// Persistent, warp-specialised W4A16 decode kernel for SEVERAL tokens (2 <= M <= 4 by dispatch, up to 8) and for bf16:
+// Persistent, warp-specialised W4A16 decode kernel for SEVERAL tokens (2 <= M <= 4) and for bf16:
 // fp16 / bf16 tensor-core MACs with the tokens in the MMA columns.  (One fp16 token is served by w4a16_decode.cu, the
 // third generation of this structure: 8 KB copies instead of the 4 KB ones below, int8-digit MACs.)
 //
@@ -68,29 +68,6 @@ struct RingArgs {
   RingLayout L;
 };
 
-__device__ __forceinline__ void ring_cp_async16(uint32_t dst, const void* src) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-}
-__device__ __forceinline__ void ring_cp_async_arrive(uint64_t* bar) {
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void ldsm4(uint32_t (&r)[4], uint32_t addr) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(addr));
-}
-__device__ __forceinline__ uint4 lds128(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ uint16_t lds16(uint32_t addr) {
-  uint16_t v;
-  asm volatile("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
-__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
 __device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 1, %0;" ::"n"(kRingCons * 32) : "memory"); }
 
 // One 128-k group of one row block, one warp: 16 (TWO) or 8 channels x 128 input channels.
@@ -236,10 +213,10 @@ __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __gri
       {  // 32 pieces of 16 B: 16 groups x 2 halves of 8 channels
         const int grp = lane >> 1, half = lane & 1;
         if (grp < ng && half * 8 < nch)
-          ring_cp_async16(smem_u32(sw) + kSlotW + pw * 512 + grp * 32 + half * 16,
-                          (pw ? szb : scb) + ((size_t)(g0 + grp) * N + n0 + half * 8) * 2);
+          cp_async<16>(smem_u32(sw) + kSlotW + pw * 512 + grp * 32 + half * 16,
+                       (pw ? szb : scb) + ((size_t)(g0 + grp) * N + n0 + half * 8) * 2);
       }
-      ring_cp_async_arrive(&full[slot]);
+      cp_async_mbar_arrive(&full[slot]);
       if (++j == nsl) j = 0, ++rb;
       if (++slot == NS) slot = 0, ++use;
     }
@@ -272,12 +249,7 @@ __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __gri
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           const int tok = tok0 + i;
-          if (tok < M && ch < nch) {
-            const uint32_t dst = map_to_rank(smem_u32(&xchg[(rb * 16 + ch) * Mp + tok]), 0);
-            asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(dst),
-                         "r"(__float_as_uint(vv[i])), "r"(dbar)
-                         : "memory");
-          }
+          if (tok < M && ch < nch) st_async_f32(map_to_rank(smem_u32(&xchg[(rb * 16 + ch) * Mp + tok]), 0), vv[i], dbar);
         }
       } else {
         if (S > 1) mbar_wait(&xch[rb], 0);
@@ -398,63 +370,22 @@ __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __gri
 // ------------------------------------------------------------------------------------ host
 namespace {
 
-int sm_count() {
-  static int cnt[32] = {};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
-  dev &= 31;
-  if (cnt[dev] == 0) {
-    int v = 0;
-    cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    cnt[dev] = v;
-  }
-  return cnt[dev];
-}
-
 constexpr int kRingSmemBudget = 113 * 1024;  // two CTAs (+ 1 KB reserved each) per 228 KB SM
 
 template <typename T, bool M1>
 int launch_ring_t(const RingArgs& a, bool pdl, cudaStream_t stream) {
-  auto kern = w4a16_ring_kernel<T, M1>;
-  static bool attr_set[32] = {};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return B200AWQ_ERR_DEVICE;
-  if (!attr_set[dev & 31]) {
-    if (cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kRingSmemBudget)) return (int)e;
-    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    attr_set[dev & 31] = true;
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(a.units * a.S));
-  cfg.blockDim = dim3(kRingThreads);
-  cfg.dynamicSmemBytes = (size_t)a.L.total;
-  cfg.stream = stream;
-  cudaLaunchAttribute attrs[2];
-  int na = 0;
-  if (a.S > 1) {
-    attrs[na].id = cudaLaunchAttributeClusterDimension;
-    attrs[na].val.clusterDim.x = (unsigned)a.S;
-    attrs[na].val.clusterDim.y = 1;
-    attrs[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  if (pdl) {
-    attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attrs[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  cfg.attrs = attrs;
-  cfg.numAttrs = na;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, a);
-  return e == cudaSuccess ? 0 : (int)e;
+  if (cudaError_t e = ensure_dyn_smem<w4a16_ring_kernel<T, M1>>(kRingSmemBudget, true)) return (int)e;
+  return launch_kernel(w4a16_ring_kernel<T, M1>, dim3((unsigned)(a.units * a.S)), dim3(kRingThreads), (size_t)a.L.total,
+                       stream, pdl, (unsigned)a.S, a);
 }
 
 }  // namespace
 
 int launch_ring(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
                 bool pdl, cudaStream_t stream) {
-  if (M < 1 || M > 8 || N % 8 || K % kGroup) return B200AWQ_ERR_SHAPE;
+  if (M < 1 || M > 4 || N % 8 || K % kGroup) return B200AWQ_ERR_SHAPE;
   const int nsm = sm_count();
+  if (nsm == 0) return B200AWQ_ERR_DEVICE;
   if (nsm < 2) return B200AWQ_ERR_SHAPE;
   const int G = K / kGroup, O = N / 8;
   RingArgs a{};
@@ -462,7 +393,7 @@ int launch_ring(const void* x, const void* qw, const void* sc, const void* sz, v
   a.M = M, a.N = N, a.K = K;
   a.S = (G >= 2 * kRingCons && nsm % 2 == 0) ? 2 : 1;
   a.units = nsm / a.S;
-  a.Mp = M <= 1 ? 1 : (M <= 2 ? 2 : (M <= 4 ? 4 : 8));
+  a.Mp = M <= 1 ? 1 : (M <= 2 ? 2 : 4);
   const int oct_max = (O + a.units - 1) / a.units;
   const int nrb_max = (oct_max + 1) / 2;
   if (nrb_max > kRingMaxRb) return B200AWQ_ERR_SHAPE;

@@ -43,12 +43,6 @@
 
 namespace b200awq {
 
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-
 // Watchdog of the fused exchange (below): a rank whose peer never delivers (peer died, mismatched launch sequence)
 // gives up after kExchangeTimeoutNs, poisons its outputs with NaN and marks the exchange dead for the rest of the
 // process, so that a broken job produces visibly wrong numbers quickly instead of spinning on the GPU for ever.
@@ -85,9 +79,6 @@ inline StreamSmem stream_smem_layout(int RO, int TT, int MODE, int M, int Kc, bo
   return L;
 }
 
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
-}
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 template <typename T, int RO, int TT>
@@ -139,8 +130,8 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
       const int which = i >= pieces;
       const int j = which ? i - pieces : i;
       const int grp = j / PPG, pc = j - grp * PPG;
-      cp_async16(reinterpret_cast<uint8_t*>(which ? zbuf : sbuf) + (grp * PPG + pc) * 16,
-                 (which ? zg : sg) + (size_t)grp * N * 2 + pc * 16);
+      cp_async<16>(reinterpret_cast<uint8_t*>(which ? zbuf : sbuf) + (grp * PPG + pc) * 16,
+                   (which ? zg : sg) + (size_t)grp * N * 2 + pc * 16);
     }
     if constexpr (MODE == 2) {  // tokens M .. 8*TT-1 do not exist: their correction terms must read as zero
       for (int i = tid + M * ngroups; i < 8 * TT * ngroups; i += kStreamThreads) xsum[i] = make_float2(0.f, 0.f);
@@ -351,12 +342,7 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
       const uint32_t dst_bar = map_to_rank(smem_u32(rbar), 0);
       for (int e = tid; e < TT * 128; e += kStreamThreads) {
         const int t = e >> 7, row = (e >> 3) & 15, tok = 8 * t + (e & 7);
-        if (tok < M && row < R) {
-          const uint32_t dst = map_to_rank(smem_u32(&rbuf[rank * TT * 128 + e]), 0);
-          asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(dst),
-                       "r"(__float_as_uint(cpart[e])), "r"(dst_bar)
-                       : "memory");
-        }
+        if (tok < M && row < R) st_async_f32(map_to_rank(smem_u32(&rbuf[rank * TT * 128 + e]), 0), cpart[e], dst_bar);
       }
     } else {
       if (tid == 0) mbar_expect_tx(rbar, (uint32_t)((S - 1) * nvalid * 4));
@@ -457,44 +443,18 @@ static int launch_stream_t(const void* x, const void* qw, const void* sc, const 
   if (pa.world > 1 && TT != 1) return B200AWQ_ERR_SHAPE;
   const StreamSmem L = stream_smem_layout(RO, TT, MODE, M, Kc, S > 1);
   if (L.total > kStreamSmemCap) return B200AWQ_ERR_SHAPE;
-  auto kern = w4a16_stream_kernel<T, RO, TT>;
-  static bool attr_set[32] = {};  // per kernel instantiation and device
-  if (cudaError_t ea = ensure_dyn_smem(kern, kStreamSmemCap, attr_set)) return (int)ea;
+  if (cudaError_t ea = ensure_dyn_smem<w4a16_stream_kernel<T, RO, TT>>(kStreamSmemCap)) return (int)ea;
   const int ctas = N / (8 * RO) * S;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)ctas);
-  cfg.blockDim = dim3(kStreamWarps * 32);
   // Co-residency: a launch that fits in one wave runs fastest with FEW CTAs per SM (the next launch's
   // CTAs only need enough room to prefetch); multi-wave launches want as many as fit (measured, DESIGN.md).
   size_t dyn = L.total;
-  int dev = 0, nsm = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
-  if (nsm <= 0) nsm = 132;
+  const int nsm = sm_count();
+  if (nsm == 0) return B200AWQ_ERR_DEVICE;
   const int per_sm = ctas <= 2 * nsm ? 2 : (ctas <= 3 * nsm ? 3 : 0);
   if (per_sm > 0 && S == 1) dyn = std::max(dyn, (size_t)(233472 / (per_sm + 1) - 512));
   if (dyn > (size_t)kStreamSmemCap) dyn = L.total;
-  cfg.dynamicSmemBytes = dyn;
-  cfg.stream = stream;
-  cudaLaunchAttribute attrs[2];
-  int na = 0;
-  if (S > 1) {
-    attrs[na].id = cudaLaunchAttributeClusterDimension;
-    attrs[na].val.clusterDim.x = S;
-    attrs[na].val.clusterDim.y = 1;
-    attrs[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  if (pdl) {
-    attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attrs[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  cfg.attrs = attrs;
-  cfg.numAttrs = na;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, (const T*)x, (const uint16_t*)qw, (const T*)sc, (const T*)sz, (T*)y, M, N,
-                                     K, Kc, S, L, pa);
-  return e == cudaSuccess ? 0 : (int)e;
+  return launch_kernel(w4a16_stream_kernel<T, RO, TT>, dim3((unsigned)ctas), dim3(kStreamWarps * 32), dyn, stream, pdl,
+                       (unsigned)S, x, qw, sc, sz, y, M, N, K, Kc, S, L, pa);
 }
 
 template <typename T>

@@ -33,13 +33,6 @@ constexpr int kBK = 64;         // k per pipeline stage
 constexpr int kWgThreads = 384;  // producer warpgroup + 2 consumer warpgroups
 constexpr int kWBytes = kBM * kBK / 2;  // 4096: packed weights per stage
 
-// keeps the compiler from moving accumulator reads / writes across a wgmma fence or wait
-template <int NA>
-__device__ __forceinline__ void acc_fence(float (&d)[NA]) {
-#pragma unroll
-  for (int i = 0; i < NA; ++i) asm volatile("" : "+f"(d[i])::"memory");
-}
-
 // D[64 x N] (+)= A[64 x 16] (registers) * B[16 x N] (shared memory, K-major), fp32 accumulate
 template <typename T>
 __device__ __forceinline__ void wgmma_rs_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accum) {
@@ -341,13 +334,6 @@ w4a16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_consta
 }
 
 // ------------------------------------------------------------------------------------ host
-static int wg_sm_count() {
-  int dev = 0, n = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  return n > 0 ? n : 132;
-}
-
 // max_clusters <= 0: one cluster per tile (all resident at once when they fit); else a persistent grid of that many
 template <typename T, int TN>
 static int launch_wgmma_t(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K,
@@ -376,35 +362,12 @@ static int launch_wgmma_t(const void* x, const void* qw, const void* sc, const v
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return B200AWQ_ERR_DRIVER;
   }
-  auto kern = w4a16_wgmma_kernel<T, TN>;
-  static bool attr_set[32] = {};  // per kernel instantiation and device
-  if (cudaError_t ea = ensure_dyn_smem(kern, L::kTotal, attr_set)) return (int)ea;
+  if (cudaError_t ea = ensure_dyn_smem<w4a16_wgmma_kernel<T, TN>>(L::kTotal)) return (int)ea;
   const int tiles = ((M + TN - 1) / TN) * (N / kBM);
   int clusters = tiles;
   if (max_clusters > 0 && max_clusters < clusters) clusters = max_clusters;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(clusters * S));
-  cfg.blockDim = dim3(kWgThreads);
-  cfg.dynamicSmemBytes = L::kTotal;
-  cfg.stream = stream;
-  cudaLaunchAttribute attrs[2];
-  int na = 0;
-  if (S > 1) {
-    attrs[na].id = cudaLaunchAttributeClusterDimension;
-    attrs[na].val.clusterDim.x = S;
-    attrs[na].val.clusterDim.y = 1;
-    attrs[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  if (pdl) {
-    attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attrs[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  cfg.attrs = attrs;
-  cfg.numAttrs = na;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, tm_x, tm_w, (const T*)sc, (const T*)sz, (T*)y, M, N, K, S);
-  return e == cudaSuccess ? 0 : (int)e;
+  return launch_kernel(w4a16_wgmma_kernel<T, TN>, dim3((unsigned)(clusters * S)), dim3(kWgThreads), (size_t)L::kTotal, stream,
+                       pdl, (unsigned)S, tm_x, tm_w, sc, sz, y, M, N, K, S);
 }
 
 template <typename T>
@@ -427,7 +390,8 @@ static int launch_wgmma(int tn, const void* x, const void* qw, const void* sc, c
 int launch_umma(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
                 bool pdl, cudaStream_t stream) {
   if (M < 1 || N % kBM || K % kGroup) return B200AWQ_ERR_SHAPE;
-  const int sms = wg_sm_count();
+  const int sms = sm_count();
+  if (sms == 0) return B200AWQ_ERR_DEVICE;
   // joint choice of the token tile and the k split by a small cost model (cycles per CTA, estimated): a 64-k stage
   // costs max(dequantisation ~400, wgmma 4 * tn + 100), a tile's epilogue ~10 tn (+6000 when the partial tiles of
   // a split are reduced over the cluster), a launch ~12000; makespan = waves x that.  A split (cluster of S CTAs on
@@ -454,9 +418,10 @@ int launch_umma(const void* x, const void* qw, const void* sc, const void* sz, v
 // whose slice is <= 512 k, or <= 1024 k once there are at least two CTAs per SM.
 int launch_flat(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
                 bool pdl, cudaStream_t stream) {
-  if (M < 1 || M > 64 || N % kBM || K % kGroup) return B200AWQ_ERR_SHAPE;
+  if (M < 1 || M > 16 || N % kBM || K % kGroup) return B200AWQ_ERR_SHAPE;
   const int groups = K / kGroup;
-  const int sms = wg_sm_count();
+  const int sms = sm_count();
+  if (sms == 0) return B200AWQ_ERR_DEVICE;
   int S = 1;
   for (int s = 1; s <= 8; ++s) {
     if (groups % s) continue;
@@ -465,8 +430,7 @@ int launch_flat(const void* x, const void* qw, const void* sc, const void* sz, v
     if (kc <= 512) break;
     if (kc <= 1024 && (N / kBM) * s >= 2 * sms) break;
   }
-  const int tn = M <= 16 ? 16 : (M <= 32 ? 32 : 64);
-  return launch_wgmma(tn, x, qw, sc, sz, y, M, N, K, dtype, pdl, 0, S, stream);
+  return launch_wgmma(16, x, qw, sc, sz, y, M, N, K, dtype, pdl, 0, S, stream);
 }
 
 }  // namespace b200awq

@@ -22,10 +22,6 @@ constexpr int kMaxThreads = 1024;
 template <int VEC>
 __host__ __device__ constexpr int chunks_per_thread() { return VEC == 8 ? 4 : 8; }
 
-template <typename T> __device__ __forceinline__ float to_f(T v);
-template <> __device__ __forceinline__ float to_f<__half>(__half v) { return __half2float(v); }
-template <> __device__ __forceinline__ float to_f<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
-
 // VEC consecutive elements (VEC = 8: one 16-byte load)
 template <int VEC, typename T>
 __device__ __forceinline__ void load_row(const T* p, T (&e)[VEC]) {
@@ -92,7 +88,7 @@ __global__ void __launch_bounds__(kMaxThreads) quant_per_token_kernel(const T* _
     if (ci < nc) {
       load_row<VEC>(x + row * n + ci * VEC, v[j]);
 #pragma unroll
-      for (int e = 0; e < VEC; ++e) amax = fmaxf(amax, fabsf(to_f(v[j][e])));
+      for (int e = 0; e < VEC; ++e) amax = fmaxf(amax, fabsf(to_float(v[j][e])));
     }
   }
   amax = block_max(amax, red);
@@ -104,7 +100,7 @@ __global__ void __launch_bounds__(kMaxThreads) quant_per_token_kernel(const T* _
     if (ci < nc) {
       int8_t c[VEC];
 #pragma unroll
-      for (int e = 0; e < VEC; ++e) c[e] = f2s8_rni_sat(fmul_ftz(to_f(v[j][e]), inv));
+      for (int e = 0; e < VEC; ++e) c[e] = f2s8_rni_sat(fmul_ftz(to_float(v[j][e]), inv));
       store_codes<VEC>(q + row * n + ci * VEC, c);
     }
   }
@@ -135,7 +131,7 @@ __global__ void __launch_bounds__(kMaxThreads) layernorm_quant_kernel(const T* _
       load_row<VEC>(x + row * n + ci * VEC, e8);
 #pragma unroll
       for (int e = 0; e < VEC; ++e) {
-        v[j][e] = to_f(e8[e]);
+        v[j][e] = to_float(e8[e]);
         sum = fadd_ftz(sum, v[j][e]);
         sq = ffma_ftz(v[j][e], v[j][e], sq);
       }
@@ -146,7 +142,7 @@ __global__ void __launch_bounds__(kMaxThreads) layernorm_quant_kernel(const T* _
   const float var = ffma_ftz(-mean, mean, fdiv_approx(sq, (float)n));
   const float rstd = frsqrt_approx(fadd_ftz(var, eps));
   const float tscale = kPerToken ? 0.f : __half2float(scale[0]);
-  float amax = to_f(from_float<T>(1e-6f));
+  float amax = to_float(from_float<T>(1e-6f));
 #pragma unroll
   for (int j = 0; j < C; ++j) {
     const int ci = threadIdx.x + j * blockDim.x;
@@ -159,9 +155,9 @@ __global__ void __launch_bounds__(kMaxThreads) layernorm_quant_kernel(const T* _
       for (int e = 0; e < VEC; ++e) {
         const float d = fmul_ftz(fsub_ftz(v[j][e], mean), rstd);
         float y;
-        if (kPerToken && beta) y = ffma_ftz(d, to_f(g8[e]), to_f(b8[e]));
-        else y = fmul_ftz(d, to_f(g8[e]));
-        const float yt = to_f(from_float<T>(y));
+        if (kPerToken && beta) y = ffma_ftz(d, to_float(g8[e]), to_float(b8[e]));
+        else y = fmul_ftz(d, to_float(g8[e]));
+        const float yt = to_float(from_float<T>(y));
         if constexpr (kPerToken) {
           amax = fmaxf(amax, fabsf(yt));
           v[j][e] = y;
@@ -246,8 +242,6 @@ __global__ void __launch_bounds__(kMaxThreads) gelu_quant_kernel(const __half* _
   }
 }
 
-bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
 // threads for a row of `chunks` accesses: one access per thread where possible, a multiple of 32
 unsigned row_threads(int chunks) {
   const int per = (chunks + kMaxThreads - 1) / kMaxThreads;
@@ -258,17 +252,7 @@ unsigned row_threads(int chunks) {
 template <typename... KArgs, typename... Args>
 int launch_rows(void (*kern)(KArgs...), int m, int chunks, bool pdl, cudaStream_t stream, Args... args) {
   if (chunks > chunks_per_thread<1>() * kMaxThreads) return B200AWQ_ERR_SHAPE;  // (16-byte rows: 4096 chunks, checked by the caller)
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)m);
-  cfg.blockDim = dim3(row_threads(chunks));
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
-  const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
-  return e == cudaSuccess ? 0 : (int)e;
+  return launch_kernel(kern, dim3((unsigned)m), dim3(row_threads(chunks)), 0, stream, pdl, 1, args...);
 }
 
 template <typename T>

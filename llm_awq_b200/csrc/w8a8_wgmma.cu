@@ -38,12 +38,6 @@ constexpr int kOutRow = kTN * 2 + 16;         // staged fp16 row (+ pad against 
 static_assert(kTM * kOutRow <= kStages * kStageBytes, "epilogue staging must fit in the pipeline buffers");
 constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 64 /*barriers*/;
 
-template <int NA>
-__device__ __forceinline__ void acc_fence_s32(int (&d)[NA]) {
-#pragma unroll
-  for (int i = 0; i < NA; ++i) asm volatile("" : "+r"(d[i])::"memory");
-}
-
 // D[64 x 128] (+)= A[64 x 32] * B[32 x 128], int8 x int8 -> int32, both operands K-major in shared memory
 __device__ __forceinline__ void wgmma_s8_n128(int (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
   asm volatile(
@@ -128,7 +122,7 @@ w8a8_wgmma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constan
       wgmma_s8_n128(acc, adesc + (uint64_t)(kk * 2), bdesc + (uint64_t)(kk * 2), (kb | kk) != 0 ? 1u : 0u);
     wgmma_commit();
     wgmma_wait<1>();  // the previous stage's wgmmas have completed: its buffers may be refilled
-    acc_fence_s32(acc);
+    acc_fence(acc);
     if (kb > 0) {
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[prev]);
@@ -137,7 +131,7 @@ w8a8_wgmma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constan
     if (++s == kStages) s = 0, ph ^= 1;
   }
   wgmma_wait<0>();
-  acc_fence_s32(acc);
+  acc_fence(acc);
 
   // ------------------------------------------------ epilogue
   pdl_wait_prior_grid();  // scales and bias may come from the previous kernel too (a no-op once the producer waited)
@@ -203,22 +197,11 @@ int launch_w8a8_gemm(const void* x, const void* w, const void* wscales, const vo
   if (int e = encode_kmajor_s8(enc, &tm_x, x, M, K, kTM)) return e;
   if (int e = encode_kmajor_s8(enc, &tm_w, w, N, K, kTN)) return e;
   auto kern = bias ? w8a8_wgmma_kernel<true> : w8a8_wgmma_kernel<false>;
-  static bool attr_set[2][32] = {};  // per instantiation and device
-  if (cudaError_t ea = ensure_dyn_smem(kern, kSmemBytes, attr_set[bias ? 1 : 0])) return (int)ea;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)((N + kTN - 1) / kTN), (unsigned)((M + kTM - 1) / kTM));
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = kSmemBytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, tm_x, tm_w, static_cast<const __half*>(wscales),
-                                     static_cast<const __half*>(ascales), static_cast<const __half*>(bias),
-                                     static_cast<__half*>(y), M, N, K);
-  return e == cudaSuccess ? 0 : (int)e;
+  const cudaError_t ea = bias ? ensure_dyn_smem<w8a8_wgmma_kernel<true>>(kSmemBytes)
+                              : ensure_dyn_smem<w8a8_wgmma_kernel<false>>(kSmemBytes);
+  if (ea) return (int)ea;
+  return launch_kernel(kern, dim3((unsigned)((N + kTN - 1) / kTN), (unsigned)((M + kTM - 1) / kTM)), dim3(kThreads),
+                       kSmemBytes, stream, pdl, 1, tm_x, tm_w, wscales, ascales, bias, y, M, N, K);
 }
 
 }  // namespace b200awq
