@@ -208,6 +208,31 @@ int b200awq_splitkv_attention(const void* q, const void* k, const void* v, void*
 size_t b200awq_splitkv_attention_workspace_bytes(int batch, int seqlen_q, int seqlen_k, int heads, int kv_heads,
                                                  int head_dim);
 
+/* Attention of a chunk of queries over a KV cache, read in place (tinychat's chunked prefill and multi-round chat:
+ * the chunk's k / v are already stored in the cache, the history is not copied out of it).  For the caller's
+ * `flash_attn_func(q, cache_k[:B, :seqlen_k], cache_v[:B, :seqlen_k], causal)` in either cache layout:
+ *   B200AWQ_KV_FT    k_cache [>= batch, kv_heads, head_dim / 8, max_len, 8], v_cache [>= batch, kv_heads, max_len,
+ *                    head_dim] (the decode caches of b200awq_single_query_attention)
+ *   B200AWQ_KV_BTHD  k_cache, v_cache [>= batch, max_len, kv_heads, head_dim] (long_forward's caches)
+ * both contiguous.  Semantics as b200awq_splitkv_attention over keys [0, seqlen_k) of cache rows [0, batch): q
+ * [batch, seqlen_q, heads, head_dim] with strides q_strides (batch, token, head) in ELEMENTS, out [batch, seqlen_q,
+ * heads, head_dim] contiguous; causal != 0 aligns the mask bottom-right (query i sees keys j <= i + seqlen_k -
+ * seqlen_q; a row that sees no key is zero).  Cache slots >= seqlen_k and cache rows >= batch are never read.
+ * Any seqlen_q >= 1; head_dim in {64, 128}, heads % kv_heads == 0, 1 <= max_len, seqlen_k <= max_len and a finite
+ * softmax_scale > 0 (else B200AWQ_ERR_SHAPE).  q, caches and out 16-byte aligned, q_strides multiples of 8
+ * (else B200AWQ_ERR_ALIGN).  batch == 0 or seqlen_q == 0 is a no-op.
+ * `workspace`: as for b200awq_splitkv_attention, >= b200awq_kv_cache_attention_workspace_bytes(...) bytes (0: the
+ * shape never splits the keys, NULL is fine), and the same per-stream buffer may serve all three attention entries.
+ * One kernel launch per call (the splits are combined inside it); deterministic; safe under graph capture. */
+#define B200AWQ_KV_FT 0
+#define B200AWQ_KV_BTHD 1
+int b200awq_kv_cache_attention(const void* q, const void* k_cache, const void* v_cache, void* out, int layout,
+                               int batch, int seqlen_q, int seqlen_k, int max_len, int heads, int kv_heads,
+                               int head_dim, const long long q_strides[3], float softmax_scale, int causal, int dtype,
+                               void* workspace, size_t workspace_bytes, void* stream);
+size_t b200awq_kv_cache_attention_workspace_bytes(int layout, int batch, int seqlen_q, int seqlen_k, int heads,
+                                                  int kv_heads, int head_dim);
+
 /* ---- W8A8 (int8 weights, int8 per-token activations): the vision-tower ops of the reference's extension
  * (csrc/pybind.cpp:30-37), called by awq/quantize/w8a8_linear.py and tinychat's QuantSiglipEncoder /
  * QuantInternVisionEncoder.  Scales are fp16 everywhere (the reference reads them as at::Half).  fp32 activations,

@@ -250,6 +250,36 @@ int b200awq_splitkv_attention(const void* q, const void* k, const void* v, void*
                  true);
 }
 
+size_t b200awq_kv_cache_attention_workspace_bytes(int layout, int batch, int seqlen_q, int seqlen_k, int heads,
+                                                  int kv_heads, int head_dim) {
+  return b200awq::kv_cache_attention_workspace_bytes(layout, batch, seqlen_q, seqlen_k, heads, kv_heads, head_dim);
+}
+
+int b200awq_kv_cache_attention(const void* q, const void* k_cache, const void* v_cache, void* out, int layout, int batch,
+                               int seqlen_q, int seqlen_k, int max_len, int heads, int kv_heads, int head_dim,
+                               const long long q_strides[3], float softmax_scale, int causal, int dtype, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+  if (int e = check_dtype(dtype)) return e;
+  if ((layout != B200AWQ_KV_FT && layout != B200AWQ_KV_BTHD) || batch < 0 || seqlen_q < 0 || seqlen_k < 0 ||
+      max_len < 1 || seqlen_k > max_len || heads < 1 || kv_heads < 1 || heads % kv_heads ||
+      (head_dim != 64 && head_dim != 128) || !(std::isfinite(softmax_scale) && softmax_scale > 0.f))
+    return B200AWQ_ERR_SHAPE;  // the softmax runs on the raw scores' max: scale > 0
+  if (!aligned16(q) || !aligned16(k_cache) || !aligned16(v_cache) || !aligned16(out) || !q_strides) return B200AWQ_ERR_ALIGN;
+  for (int i = 0; i < 3; ++i)
+    if (q_strides[i] % 8) return B200AWQ_ERR_ALIGN;  // Q is read in 16-byte pieces
+  if (workspace && !aligned16(workspace)) return B200AWQ_ERR_ALIGN;
+  if (workspace_bytes < b200awq::kv_cache_attention_workspace_bytes(layout, batch, seqlen_q, seqlen_k, heads, kv_heads,
+                                                                    head_dim) ||
+      (workspace_bytes && !workspace))
+    return B200AWQ_ERR_WORKSPACE;
+  if (batch == 0 || seqlen_q == 0) return 0;
+  if (int e = check_device()) return e;
+  return counted(b200awq::launch_kv_cache_attention(q, k_cache, v_cache, out, layout, batch, seqlen_q, seqlen_k, max_len, heads,
+                                                    kv_heads, head_dim, q_strides, softmax_scale, causal != 0, dtype,
+                                                    workspace, workspace_bytes, static_cast<cudaStream_t>(stream)),
+                 true);
+}
+
 int b200awq_rope_with_pos(const void* x, const float* freqs, void* y, int s, int b, int h, int d, int d2,
                           const long long in_strides[4], const long long out_strides[4], int dtype, void* stream) {
   if (int e = check_dtype(dtype)) return e;

@@ -484,6 +484,53 @@ torch::Tensor flash_attn_varlen_qkvpacked_func(const torch::Tensor& qkv, const t
                                (int)cu_seqlens.numel() - 1, (int)max_seqlen, (int)max_seqlen, softmax_scale, causal);
 }
 
+// Attention of a chunk q [B, Sq, H, D] over keys [0, seqlen_k) of a KV cache, read in place -> out [B, Sq, H, D].  The
+// layout follows from k_cache: 5-D is tinychat's decode cache (k_cache [Bc, Hkv, D / 8, Lmax, 8], v_cache [Bc, Hkv,
+// Lmax, D]), 4-D long_forward's ([Bc, Lmax, Hkv, D] both); Bc >= B, caches contiguous.  q may be a strided view (as for
+// flash_attn_func, one that the kernel cannot read is copied contiguous first).
+torch::Tensor kv_cache_attention(const torch::Tensor& q_in, const torch::Tensor& k_cache, const torch::Tensor& v_cache,
+                                 int64_t seqlen_k, c10::optional<double> softmax_scale, bool causal) {
+  const char* fn = "kv_cache_attention";
+  check_attention_args(q_in, k_cache, v_cache, 0.0, fn);
+  TORCH_CHECK(q_in.dim() == 4, fn, ": q must be [batch, seqlen_q, heads, head_dim]");
+  TORCH_CHECK(k_cache.is_contiguous() && v_cache.is_contiguous(), fn, ": caches must be contiguous");
+  TORCH_CHECK(k_cache.device() == q_in.device() && v_cache.device() == q_in.device(), fn, ": tensors must be on one device");
+  const int64_t d = q_in.size(3);
+  int layout, kv_heads;
+  int64_t rows, max_len;
+  if (k_cache.dim() == 5) {
+    layout = B200AWQ_KV_FT;
+    rows = k_cache.size(0), kv_heads = (int)k_cache.size(1), max_len = k_cache.size(3);
+    TORCH_CHECK(k_cache.size(2) * 8 == d && k_cache.size(4) == 8, fn, ": k_cache must be [batch, kv_heads, head_dim / 8, max_len, 8]");
+    TORCH_CHECK(v_cache.dim() == 4 && v_cache.sizes() == torch::IntArrayRef({rows, kv_heads, max_len, d}), fn,
+                ": v_cache must be [batch, kv_heads, max_len, head_dim]");
+  } else {
+    TORCH_CHECK(k_cache.dim() == 4, fn, ": k_cache must be 5-D (FasterTransformer layout) or 4-D [batch, max_len, kv_heads, head_dim]");
+    layout = B200AWQ_KV_BTHD;
+    rows = k_cache.size(0), max_len = k_cache.size(1), kv_heads = (int)k_cache.size(2);
+    TORCH_CHECK(k_cache.size(3) == d && v_cache.sizes() == k_cache.sizes(), fn, ": k_cache / v_cache must be [batch, max_len, kv_heads, head_dim]");
+  }
+  TORCH_CHECK(q_in.size(0) <= rows, fn, ": q has ", q_in.size(0), " batch rows, the caches ", rows);
+  TORCH_CHECK(seqlen_k >= 0 && seqlen_k <= max_len, fn, ": seqlen_k must be in [0, ", max_len, "]");
+  TORCH_CHECK(max_len <= INT32_MAX && q_in.size(1) <= INT32_MAX, fn, ": sizes out of range");
+  const c10::cuda::CUDAGuard guard(q_in.device());
+  const torch::Tensor q = tma_ready(q_in);
+  const int batch = (int)q.size(0), seqlen_q = (int)q.size(1), heads = (int)q.size(2);
+  torch::Tensor out = torch::empty({q.size(0), q.size(1), q.size(2), d}, q.options());
+  const float scale = softmax_scale.has_value() ? (float)softmax_scale.value() : 1.0f / std::sqrt((float)d);
+  const long long qs[3] = {q.stride(0), q.stride(1), q.stride(2)};
+  const int dt = q.scalar_type() == at::ScalarType::Half ? B200AWQ_DTYPE_F16 : B200AWQ_DTYPE_BF16;
+  const size_t need =
+      b200awq_kv_cache_attention_workspace_bytes(layout, batch, seqlen_q, (int)seqlen_k, heads, kv_heads, (int)d);
+  const torch::Tensor* ws = need ? &attention_workspace(q, need) : nullptr;
+  raise(b200awq_kv_cache_attention(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), out.data_ptr(), layout, batch, seqlen_q,
+                                   (int)seqlen_k, (int)max_len, heads, kv_heads, (int)d, qs, scale, causal ? 1 : 0, dt,
+                                   ws ? ws->data_ptr() : nullptr, ws ? (size_t)ws->numel() : 0,
+                                   at::cuda::getCurrentCUDAStream().stream()),
+        false);
+  return out;
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "H100 (sm_90a) drop-in for llm-awq's awq_inference_engine (W4A16 and W8A8 paths)";
   m.def("gemm_forward_cuda_new", &gemm_forward_cuda_new, "New quantized GEMM kernel.");
@@ -512,6 +559,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         "Attention over packed sequences of a fused qkv tensor (flash-attn's flash_attn_varlen_qkvpacked_func)",
         py::arg("qkv"), py::arg("cu_seqlens"), py::arg("max_seqlen"), py::arg("dropout_p") = 0.0,
         py::arg("softmax_scale") = py::none(), py::arg("causal") = false);
+  m.def("kv_cache_attention", &kv_cache_attention,
+        "Attention of a chunk of queries over a KV cache in either of tinychat's layouts, read in place", py::arg("q"),
+        py::arg("k_cache"), py::arg("v_cache"), py::arg("seqlen_k"), py::arg("softmax_scale") = py::none(),
+        py::arg("causal") = true);
   m.def("set_pdl", [](bool on) { return b200awq_set_pdl(on ? 1 : 0) != 0; }, "programmatic dependent launch on/off");
   m.def("launch_count", []() { return b200awq_launch_count(); }, "kernels launched by libb200awq so far");
   m.def("version", []() { return std::string(b200awq_version()); });

@@ -153,6 +153,13 @@ int launch_splitkv_attention(const void* q, const void* k, const void* v, void* 
                              int heads, int kv_heads, int head_dim, const long long* q_strides, const long long* k_strides,
                              const long long* v_strides, float softmax_scale, bool causal, int dtype, void* workspace,
                              size_t workspace_bytes, cudaStream_t stream);
+// the same kernel over a KV cache in either of tinychat's layouts, any seqlen_q; arguments as b200awq_kv_cache_attention
+size_t kv_cache_attention_workspace_bytes(int layout, int batch, int seqlen_q, int seqlen_k, int heads, int kv_heads,
+                                          int head_dim);
+int launch_kv_cache_attention(const void* q, const void* k_cache, const void* v_cache, void* out, int layout, int batch,
+                              int seqlen_q, int seqlen_k, int max_len, int heads, int kv_heads, int head_dim,
+                              const long long* q_strides, float softmax_scale, bool causal, int dtype, void* workspace,
+                              size_t workspace_bytes, cudaStream_t stream);
 
 // the same kernel for skinny batches, 1 <= M <= 16, N % 128 == 0: one CTA per tile and k slice (w4a16_wgmma.cu)
 int launch_flat(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
