@@ -68,6 +68,19 @@ int b200awq_w4a16_gemm(const void* x, const void* qweight, const void* scales, c
 
 size_t b200awq_w4a16_gemm_workspace_bytes(int m, int n, int k);
 
+/* The quantised linear with its bias and residual adds in the same launch:
+ *   y[i, j] = rn_T( rn_T( rn_T(acc[i, j]) + bias[j] ) + residual[i, j] )
+ * with acc the sum of b200awq_w4a16_gemv / gemm and each + done in fp32 and rounded once to T: bit-identical to those
+ * entries followed by PyTorch's `out + bias`, then `residual + out` (WQLinear.forward, awq/quantize/qmodule.py:221,
+ * and the decoder blocks' `residual + x`).  Either operand may be NULL; with both NULL this launches exactly what
+ * gemv / gemm launch.  bias [n] and residual [m, n] (row-major) are of the activation dtype, 16-byte aligned, and
+ * must not overlap y.  The reference's dispatch rule (qmodule.py:206): m < 8 takes the gemv routes (n % 8 == 0),
+ * m >= 8 the gemm routes (n % 128 == 0).  bias and residual are read only after the launch's dependency wait, so
+ * either may be written by the launch right before it in the stream.  One launch, no workspace, deterministic. */
+int b200awq_w4a16_linear(const void* x, const void* qweight, const void* scales, const void* szeros,
+                         const void* bias, const void* residual, void* y, int m, int n, int k, int group_size,
+                         int dtype, void* stream);
+
 /* Row-parallel tensor parallelism (new work, SURVEY.md §8e; the reference has no multi-GPU path): the decode
  * GEMV of THIS rank's k-slice fused with the sum all-reduce of the [m, n] partial outputs over NVLink peer
  * memory, in one kernel.  Every rank calls it with its own shard and the same (m, n); on return (stream order)

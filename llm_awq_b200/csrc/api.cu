@@ -77,12 +77,19 @@ int check_device() {
   return v == 1 ? 0 : B200AWQ_ERR_DEVICE;
 }
 
-int check_common(const void* x, const void* qw, const void* sc, const void* sz, void* y, int m, int n, int k,
-                 int group_size, int dtype) {
+// the W4A16 entries' argument checks that need no device
+int check_args(const void* x, const void* qw, const void* sc, const void* sz, void* y, int m, int n, int k, int group_size,
+               int dtype) {
   if (int e = check_dtype(dtype)) return e;
   if (group_size != 128) return B200AWQ_ERR_GROUP;
   if (m < 1 || n < 8 || k < 128 || (n % 8) || (k % 128)) return B200AWQ_ERR_SHAPE;
   if (!aligned16(x) || !aligned16(qw) || !aligned16(sc) || !aligned16(sz) || !aligned16(y)) return B200AWQ_ERR_ALIGN;
+  return 0;
+}
+
+int check_common(const void* x, const void* qw, const void* sc, const void* sz, void* y, int m, int n, int k,
+                 int group_size, int dtype) {
+  if (int e = check_args(x, qw, sc, sz, y, m, n, k, group_size, dtype)) return e;
   return check_device();
 }
 
@@ -105,13 +112,29 @@ bool use_flat(int m, int n, int k) {
 // Small token counts (decode and the bottom of the batch sweep): decode (one token) -> ring -> flat -> stream, each returning
 // B200AWQ_ERR_SHAPE (or, for the cluster kernels, a launch-configuration error) when it cannot take the shape.
 int launch_small(const void* x, const void* qw, const void* sc, const void* sz, void* y, int m, int n, int k, int dtype,
-                 cudaStream_t st) {
+                 cudaStream_t st, const b200awq::Epilogue& epi = {}) {
   int r = B200AWQ_ERR_SHAPE;
   if (use_decode(m, dtype))
-    r = next_on_config_error(b200awq::launch_decode(x, qw, sc, sz, y, n, k, dtype, pdl_enabled(), decode_tuning(), st));
-  if (r != 0 && m <= kRingMaxM) r = next_on_config_error(b200awq::launch_ring(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st));
-  if (r != 0 && use_flat(m, n, k)) r = next_on_config_error(b200awq::launch_flat(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st));
-  if (r != 0 && m <= kStreamMaxM) r = b200awq::launch_stream(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st);
+    r = next_on_config_error(b200awq::launch_decode(x, qw, sc, sz, y, n, k, dtype, pdl_enabled(), decode_tuning(), st, epi));
+  if (r != 0 && m <= kRingMaxM)
+    r = next_on_config_error(b200awq::launch_ring(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st, epi));
+  if (r != 0 && use_flat(m, n, k))
+    r = next_on_config_error(b200awq::launch_flat(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st, epi));
+  if (r != 0 && m <= kStreamMaxM) r = b200awq::launch_stream(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st, nullptr, epi);
+  return r;
+}
+
+// Routing of b200awq_w4a16_gemm (and of b200awq_w4a16_linear from 8 tokens): the small-token kernels, else the wgmma tile
+// kernel.  n % 128 == 0.
+int launch_gemm(const void* x, const void* qw, const void* sc, const void* sz, void* y, int m, int n, int k, int dtype,
+                cudaStream_t st, const b200awq::Epilogue& epi = {}) {
+  int r = B200AWQ_ERR_SHAPE;
+  // 9..16 tokens on the large layers (>= 48 M weights): the persistent tile launch (split-k); everything else below
+  // 17 tokens: the small-token kernels
+  const bool big_mid = m > 8 && (long long)n * k >= 48ll * 1000 * 1000;
+  if (m <= 16 && !big_mid) r = launch_small(x, qw, sc, sz, y, m, n, k, dtype, st, epi);
+  if (r == B200AWQ_ERR_SHAPE)  // 128-channel wgmma tiles; split-k over a cluster for small token counts
+    r = b200awq::launch_umma(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st, epi);
   return r;
 }
 
@@ -124,6 +147,20 @@ int b200awq_w4a16_gemv(const void* x, const void* qweight, const void* scales, c
   if (int e = check_common(x, qweight, scales, szeros, y, m, n, k, group_size, dtype)) return e;
   if (m > 7) return B200AWQ_ERR_BATCH;  // reference envelope: gemv_cuda.cu:291-330
   return counted(launch_small(x, qweight, scales, szeros, y, m, n, k, dtype, static_cast<cudaStream_t>(stream)), true);
+}
+
+int b200awq_w4a16_linear(const void* x, const void* qweight, const void* scales, const void* szeros, const void* bias,
+                         const void* residual, void* y, int m, int n, int k, int group_size, int dtype, void* stream) {
+  if (int e = check_args(x, qweight, scales, szeros, y, m, n, k, group_size, dtype)) return e;
+  if ((bias && !aligned16(bias)) || (residual && !aligned16(residual))) return B200AWQ_ERR_ALIGN;
+  if (m >= 8 && n % 128) return B200AWQ_ERR_SHAPE;  // the GEMM envelope (b200awq_w4a16_gemm)
+  if (int e = check_device()) return e;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const b200awq::Epilogue epi{bias, residual};
+  // the reference's dispatch rule (awq/quantize/qmodule.py:206): the GEMV's routes below 8 tokens, the GEMM's from 8
+  return counted(m < 8 ? launch_small(x, qweight, scales, szeros, y, m, n, k, dtype, st, epi)
+                       : launch_gemm(x, qweight, scales, szeros, y, m, n, k, dtype, st, epi),
+                 true);
 }
 
 int b200awq_w4a16_gemv_allreduce(const void* x, const void* qweight, const void* scales, const void* szeros, void* y, int m,
@@ -318,14 +355,7 @@ int b200awq_w4a16_gemm(const void* x, const void* qweight, const void* scales, c
   (void)workspace_bytes;
   if (int e = check_common(x, qweight, scales, szeros, y, m, n, k, group_size, dtype)) return e;
   if (n % 128) return B200AWQ_ERR_SHAPE;  // reference: N / CTA_N with CTA_N = 128, gemm_cuda.cu:38,1225
-  int r = B200AWQ_ERR_SHAPE;
-  // 9..16 tokens on the large layers (>= 48 M weights): the persistent tile launch (split-k); everything else below
-  // 17 tokens: the small-token kernels
-  const bool big_mid = m > 8 && (long long)n * k >= 48ll * 1000 * 1000;
-  if (m <= 16 && !big_mid) r = launch_small(x, qweight, scales, szeros, y, m, n, k, dtype, static_cast<cudaStream_t>(stream));
-  if (r == B200AWQ_ERR_SHAPE)  // 128-channel wgmma tiles; split-k over a cluster for small token counts
-    r = b200awq::launch_umma(x, qweight, scales, szeros, y, m, n, k, dtype, pdl_enabled(), static_cast<cudaStream_t>(stream));
-  return counted(r, true);
+  return counted(launch_gemm(x, qweight, scales, szeros, y, m, n, k, dtype, static_cast<cudaStream_t>(stream)), true);
 }
 
 // ---------------------------------------------------------------- W8A8

@@ -91,6 +91,47 @@ torch::Tensor gemm_forward_cuda_new(torch::Tensor _in_feats, torch::Tensor _kern
   return out;
 }
 
+// New entry (no counterpart in the reference's extension): WQLinear.forward's engine call with its `out + bias`
+// (awq/quantize/qmodule.py:205-221) and the decoder block's `residual + out` in one launch, bit-identical to the
+// engine call followed by those two adds.  The reference's dispatch rule picks the GEMV (m < 8) or GEMM routes.
+// bias [N] and residual (the output's shape) must have in_feats' dtype and device and be contiguous.
+torch::Tensor w4a16_linear_forward_cuda(torch::Tensor _in_feats, torch::Tensor _kernel, torch::Tensor _scales,
+                                        torch::Tensor _zeros, int64_t group_size, c10::optional<torch::Tensor> bias,
+                                        c10::optional<torch::Tensor> residual) {
+  const char* fn = "w4a16_linear_forward_cuda";
+  check_inputs(_in_feats, _kernel, _scales, _zeros);
+  const int dt = dtype_code(_in_feats, fn);
+  const int64_t k = _in_feats.size(-1);
+  const int64_t n = _kernel.size(0) * 4;
+  const int64_t m = k ? _in_feats.numel() / k : 0;
+  TORCH_CHECK(_kernel.size(1) == k, "qweight does not match in_feats");
+  TORCH_CHECK(_scales.size(1) == n && _zeros.size(1) == n && _scales.size(0) * group_size >= k &&
+                  _zeros.size(0) * group_size >= k,
+              "scales / zeros do not match (n, k, group)");
+  std::vector<int64_t> output_shape = _in_feats.sizes().vec();
+  output_shape.back() = n;
+  for (const c10::optional<torch::Tensor>* t : {&bias, &residual}) {
+    if (!t->has_value()) continue;
+    const torch::Tensor& v = t->value();
+    TORCH_CHECK(v.is_cuda() && v.device() == _in_feats.device(), fn, ": bias / residual must be on in_feats' device");
+    TORCH_CHECK(v.scalar_type() == _in_feats.scalar_type(), fn, ": bias / residual must have in_feats' dtype");
+    TORCH_CHECK(v.is_contiguous(), fn, ": bias / residual must be contiguous");
+  }
+  if (bias.has_value()) TORCH_CHECK(bias->dim() == 1 && bias->size(0) == n, fn, ": bias must be [", n, "]");
+  if (residual.has_value())
+    TORCH_CHECK(residual->sizes() == torch::IntArrayRef(output_shape), fn, ": residual must have the output's shape ",
+                torch::IntArrayRef(output_shape));
+  const c10::cuda::CUDAGuard guard(_in_feats.device());
+  at::Tensor out = torch::empty(output_shape, _in_feats.options());
+  if (m == 0) return out;
+  raise(b200awq_w4a16_linear(_in_feats.data_ptr(), _kernel.data_ptr(), _scales.data_ptr(), _zeros.data_ptr(),
+                             bias.has_value() ? bias->data_ptr() : nullptr,
+                             residual.has_value() ? residual->data_ptr() : nullptr, out.data_ptr(), (int)m, (int)n, (int)k,
+                             (int)group_size, dt, at::cuda::getCurrentCUDAStream().stream()),
+        false);
+  return out;
+}
+
 // New entry (no counterpart in the reference's extension): the whole of QuantLlamaMLP.our_llama_mlp
 // (tinychat/modules/fused_mlp.py:36-83) in one call.  The zeros tensors are used as given.
 torch::Tensor mlp_front_forward_cuda(torch::Tensor _in_feats, torch::Tensor _gate_kernel, torch::Tensor _gate_scales,
@@ -543,6 +584,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fused_rope_with_pos_forward_func", &fused_rope_with_pos_forward_func,
         "Fused rope forward function with B,S,D embedding");
   m.def("rotary_embedding_neox", &rotary_embedding_neox, "Apply GPT-NeoX style rotary embedding to query and key");
+  m.def("w4a16_linear_forward_cuda", &w4a16_linear_forward_cuda,
+        "W4A16 linear with the bias and residual adds in the same launch", py::arg("in_feats"), py::arg("kernel"),
+        py::arg("scales"), py::arg("zeros"), py::arg("group_size"), py::arg("bias") = py::none(),
+        py::arg("residual") = py::none());
   m.def("mlp_front_forward_cuda", &mlp_front_forward_cuda, "silu(x Wgate^T) * (x Wup^T) for W4A16 weights, one call");
   m.def("w8a8_gemm_forward_cuda", &w8a8_gemm_forward_cuda, "our w8a8 gemm kernel");
   m.def("w8a8_gemm_fuse_bias_forward_cuda", &w8a8_gemm_fuse_bias_forward_cuda, "our w8a8 gemm fused bias kernel");

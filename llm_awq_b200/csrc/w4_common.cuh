@@ -114,6 +114,17 @@ __device__ __forceinline__ float to_float(T v);
 template <> __device__ __forceinline__ float to_float<__half>(__half v) { return __half2float(v); }
 template <> __device__ __forceinline__ float to_float<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
 
+// Bias / residual epilogue of a W4A16 output element, after the plain store's rounding v = rn_T(acc): + bias[n], then
+// + residual[i] (the element's index in y), each add in fp32 and rounded once to T -- PyTorch's add for fp16 / bf16, in
+// tinychat's order (`out + bias`, then `residual + out`).  Either pointer may be null.  Callers load after
+// griddepcontrol.wait only: the residual is usually written by a launch shortly before in the same stream.
+template <typename T>
+__device__ __forceinline__ T add_epilogue(T v, const T* bias, const T* residual, size_t n, size_t i) {
+  if (bias) v = from_float<T>(to_float<T>(v) + to_float<T>(bias[n]));
+  if (residual) v = from_float<T>(to_float<T>(residual[i]) + to_float<T>(v));
+  return v;
+}
+
 // keeps the compiler from moving accumulator reads / writes across a wgmma fence or wait
 template <int NA>
 __device__ __forceinline__ void acc_fence(float (&d)[NA]) {

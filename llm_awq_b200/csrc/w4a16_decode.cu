@@ -116,6 +116,8 @@ struct DecArgs {
   int NS;       // ring slots
   int nrb_max;  // most row blocks any CTA owns
   DecLayout L;
+  const void* bias;      // EPI: [N] or null
+  const void* residual;  // EPI: [1, N] or null
 };
 
 __device__ __forceinline__ void dec_sts8(uint32_t addr, int v) {
@@ -139,8 +141,10 @@ __device__ __forceinline__ T silu_mul_rounded(float gate_acc, float up_acc) {
 
 // FUSED = false: y = x W~^T.   FUSED = true: y = silu(x Wgate~^T) * (x Wup~^T), both weight sets walked row block by row
 // block through the same ring (SURVEY.md §8f-1: one read of x, two weight streams, one [1, n] write).
-template <bool FUSED>
+// EPI (not with FUSED): the finisher adds a.bias / a.residual to each stored value (add_epilogue).
+template <bool FUSED, bool EPI>
 __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(const __grid_constant__ DecArgs a) {
+  static_assert(!(FUSED && EPI), "the fused MLP front has no epilogue");
   using T = __half;
   constexpr int NT = FUSED ? 2 : 1;   // weight sets
   constexpr int RW = 16 * NT;         // partial sums per row block and warp
@@ -345,6 +349,10 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
       if (FUSED) {
         const float up = __shfl_down_sync(0xffffffffu, v, 16);
         if (lane < nch) y[n0 + ch] = silu_mul_rounded<T>(v, up);
+      } else if (EPI) {  // the finisher passed griddepcontrol.wait above: bias / residual are in stream order
+        if (lane < nch)
+          y[n0 + ch] = add_epilogue<T>(from_float<T>(v), static_cast<const T*>(a.bias), static_cast<const T*>(a.residual),
+                                       (size_t)(n0 + ch), (size_t)(n0 + ch));
       } else {
         if (lane < nch) y[n0 + ch] = from_float<T>(v);
       }
@@ -585,7 +593,8 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
 // ------------------------------------------------------------------------------------ host
 namespace {
 int launch_decode_impl(const void* x, const void* qw, const void* sc, const void* sz, const void* qw2, const void* sc2,
-                       const void* sz2, void* y, int N, int K, int dtype, bool pdl, const DecodeTuning& tune, cudaStream_t stream) {
+                       const void* sz2, void* y, int N, int K, int dtype, bool pdl, const DecodeTuning& tune, cudaStream_t stream,
+                       const Epilogue& epi) {
   const bool fused = qw2 != nullptr;
   const int nt = fused ? 2 : 1;
   if (dtype != B200AWQ_DTYPE_F16 || N % 8 || K % kGroup) return B200AWQ_ERR_SHAPE;
@@ -595,6 +604,7 @@ int launch_decode_impl(const void* x, const void* qw, const void* sc, const void
   DecArgs a{};
   a.x = x, a.qw = static_cast<const uint16_t*>(qw), a.sc = sc, a.sz = sz, a.y = y;
   a.qw2 = static_cast<const uint16_t*>(qw2), a.sc2 = sc2, a.sz2 = sz2;
+  a.bias = epi.bias, a.residual = epi.residual;
   a.N = N, a.K = K;
   // k split: only when the rows alone cannot balance the SMs (efficiency of dealing Q quad rows to nsm CTAs below
   // ~0.9) and the halves still make copies of >= 4 KB; or when the digits of the whole k range would crowd out the ring
@@ -640,24 +650,28 @@ int launch_decode_impl(const void* x, const void* qw, const void* sc, const void
 
   const dim3 grid((unsigned)(a.units * a.S)), block((unsigned)((kDecCons + 2) * 32));
   if (fused) {
-    if (cudaError_t e = ensure_dyn_smem<w4a16_decode_kernel<true>>(kDecSmemBudget, true)) return (int)e;
-    return launch_kernel(w4a16_decode_kernel<true>, grid, block, (size_t)L.total, stream, pdl, (unsigned)a.S, a);
+    if (cudaError_t e = ensure_dyn_smem<w4a16_decode_kernel<true, false>>(kDecSmemBudget, true)) return (int)e;
+    return launch_kernel(w4a16_decode_kernel<true, false>, grid, block, (size_t)L.total, stream, pdl, (unsigned)a.S, a);
   }
-  if (cudaError_t e = ensure_dyn_smem<w4a16_decode_kernel<false>>(kDecSmemBudget, true)) return (int)e;
-  return launch_kernel(w4a16_decode_kernel<false>, grid, block, (size_t)L.total, stream, pdl, (unsigned)a.S, a);
+  if (epi.on()) {
+    if (cudaError_t e = ensure_dyn_smem<w4a16_decode_kernel<false, true>>(kDecSmemBudget, true)) return (int)e;
+    return launch_kernel(w4a16_decode_kernel<false, true>, grid, block, (size_t)L.total, stream, pdl, (unsigned)a.S, a);
+  }
+  if (cudaError_t e = ensure_dyn_smem<w4a16_decode_kernel<false, false>>(kDecSmemBudget, true)) return (int)e;
+  return launch_kernel(w4a16_decode_kernel<false, false>, grid, block, (size_t)L.total, stream, pdl, (unsigned)a.S, a);
 }
 }  // namespace
 
 int launch_decode(const void* x, const void* qw, const void* sc, const void* sz, void* y, int N, int K, int dtype, bool pdl,
-                  const DecodeTuning& tune, cudaStream_t stream) {
-  return launch_decode_impl(x, qw, sc, sz, nullptr, nullptr, nullptr, y, N, K, dtype, pdl, tune, stream);
+                  const DecodeTuning& tune, cudaStream_t stream, const Epilogue& epi) {
+  return launch_decode_impl(x, qw, sc, sz, nullptr, nullptr, nullptr, y, N, K, dtype, pdl, tune, stream, epi);
 }
 
 int launch_decode_mlp_front(const void* x, const void* gqw, const void* gsc, const void* gsz, const void* uqw, const void* usc,
                             const void* usz, void* y, int N, int K, int dtype, bool pdl, const DecodeTuning& tune,
                             cudaStream_t stream) {
   if (!uqw || !usc || !usz) return B200AWQ_ERR_ALIGN;
-  return launch_decode_impl(x, gqw, gsc, gsz, uqw, usc, usz, y, N, K, dtype, pdl, tune, stream);
+  return launch_decode_impl(x, gqw, gsc, gsz, uqw, usc, usz, y, N, K, dtype, pdl, tune, stream, Epilogue{});
 }
 
 }  // namespace b200awq

@@ -87,18 +87,27 @@ struct PeerArgs {
   int tok_cap;                  // tokens a region is laid out for: word slot = channel * tok_cap + token
 };
 
-// HBM-bound streaming kernel, 1 <= M <= 16 (w4a16_stream.cu)
+// Bias / residual epilogue of a W4A16 launch (b200awq_w4a16_linear): y = rn_T(rn_T(rn_T(acc) + bias[n]) + residual[i, n]),
+// either pointer may be null.  Both null (the default) launches the plain instantiation of the kernel, the one the
+// other entries run; otherwise the launcher picks the instantiation that loads them after griddepcontrol.wait.
+struct Epilogue {
+  const void* bias = nullptr;      // [N] of the activation dtype
+  const void* residual = nullptr;  // [M, N] of the activation dtype
+  bool on() const { return bias || residual; }
+};
+
+// HBM-bound streaming kernel, 1 <= M <= 16 (w4a16_stream.cu); the epilogue does not apply to the all-reduce (peers)
 int launch_stream(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                  bool pdl, cudaStream_t stream, const PeerArgs* peers = nullptr);
+                  bool pdl, cudaStream_t stream, const PeerArgs* peers = nullptr, const Epilogue& epi = Epilogue{});
 
 // TMA + wgmma tensor-core kernel, any M, N % 128 == 0 (w4a16_wgmma.cu)
 int launch_umma(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                bool pdl, cudaStream_t stream);
+                bool pdl, cudaStream_t stream, const Epilogue& epi = Epilogue{});
 
 // persistent warp-specialised decode kernel, 1 <= M <= 4 (w4a16_ring.cu); returns B200AWQ_ERR_SHAPE when the
 // activations do not fit next to a useful ring (the caller falls back to the kernels below)
 int launch_ring(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                bool pdl, cudaStream_t stream);
+                bool pdl, cudaStream_t stream, const Epilogue& epi = Epilogue{});
 
 // Test-only override of the decode kernel's plan (env B200AWQ_DECODE_SPLIT / B200AWQ_DECODE_SLOTS, api.cu): the
 // default-constructed value means "pick from the shape".
@@ -110,7 +119,7 @@ struct DecodeTuning {
 // one-token fp16 decode kernel: 8 KB bulk copies, int8-digit tensor-core MACs (w4a16_decode.cu); returns
 // B200AWQ_ERR_SHAPE for bf16 and when the activations do not fit next to a useful ring (the caller falls back)
 int launch_decode(const void* x, const void* qw, const void* sc, const void* sz, void* y, int N, int K, int dtype, bool pdl,
-                  const DecodeTuning& tune, cudaStream_t stream);
+                  const DecodeTuning& tune, cudaStream_t stream, const Epilogue& epi = Epilogue{});
 
 // one-token fused MLP front half: y = silu(x Wgate~^T) * (x Wup~^T), both weight sets through one ring (w4a16_decode.cu)
 int launch_decode_mlp_front(const void* x, const void* gqw, const void* gsc, const void* gsz, const void* uqw, const void* usc,
@@ -163,7 +172,7 @@ int launch_kv_cache_attention(const void* q, const void* k_cache, const void* v_
 
 // the same kernel for skinny batches, 1 <= M <= 16, N % 128 == 0: one CTA per tile and k slice (w4a16_wgmma.cu)
 int launch_flat(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                bool pdl, cudaStream_t stream);
+                bool pdl, cudaStream_t stream, const Epilogue& epi = Epilogue{});
 
 // RMSNorm over the last dimension, one CTA per row (rmsnorm.cu)
 int launch_rmsnorm(const void* x, const void* gamma, void* y, float eps, int m, int n, int dtype, bool pdl, cudaStream_t stream);

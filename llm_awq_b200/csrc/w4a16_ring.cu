@@ -66,6 +66,8 @@ struct RingArgs {
   int NS;     // ring slots
   int Mp;     // power of two >= M
   RingLayout L;
+  const void* bias;      // EPI: [N] or null
+  const void* residual;  // EPI: [M, N] or null
 };
 
 __device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 1, %0;" ::"n"(kRingCons * 32) : "memory"); }
@@ -136,7 +138,8 @@ __device__ __forceinline__ void group_step(uint32_t wsrc, uint32_t xsrc, uint32_
   }
 }
 
-template <typename T, bool M1>
+// EPI: the finisher adds a.bias / a.residual to each stored value (add_epilogue)
+template <typename T, bool M1, bool EPI>
 __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __grid_constant__ RingArgs a) {
   constexpr int MODE = TypeTraits<T>::kIsBf16 ? 0 : 2;  // see the header comment
   extern __shared__ __align__(128) uint8_t smem[];
@@ -259,7 +262,12 @@ __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __gri
           if (tok < M && ch < nch) {
             float r = vv[i];
             if (S > 1) r += xchg[(rb * 16 + ch) * Mp + tok];
-            y[(size_t)tok * N + n0 + ch] = from_float<T>(r);
+            const size_t i = (size_t)tok * N + n0 + ch;
+            if (EPI)  // after griddepcontrol.wait (above): bias / residual are in stream order
+              y[i] = add_epilogue<T>(from_float<T>(r), static_cast<const T*>(a.bias), static_cast<const T*>(a.residual),
+                                     (size_t)(n0 + ch), i);
+            else
+              y[i] = from_float<T>(r);
           }
         }
       }
@@ -372,17 +380,22 @@ namespace {
 
 constexpr int kRingSmemBudget = 113 * 1024;  // two CTAs (+ 1 KB reserved each) per 228 KB SM
 
-template <typename T, bool M1>
+template <typename T, bool M1, bool EPI>
 int launch_ring_t(const RingArgs& a, bool pdl, cudaStream_t stream) {
-  if (cudaError_t e = ensure_dyn_smem<w4a16_ring_kernel<T, M1>>(kRingSmemBudget, true)) return (int)e;
-  return launch_kernel(w4a16_ring_kernel<T, M1>, dim3((unsigned)(a.units * a.S)), dim3(kRingThreads), (size_t)a.L.total,
+  if (cudaError_t e = ensure_dyn_smem<w4a16_ring_kernel<T, M1, EPI>>(kRingSmemBudget, true)) return (int)e;
+  return launch_kernel(w4a16_ring_kernel<T, M1, EPI>, dim3((unsigned)(a.units * a.S)), dim3(kRingThreads), (size_t)a.L.total,
                        stream, pdl, (unsigned)a.S, a);
+}
+
+template <typename T, bool EPI>
+int launch_ring_m(const RingArgs& a, bool pdl, cudaStream_t stream) {
+  return a.M == 1 ? launch_ring_t<T, true, EPI>(a, pdl, stream) : launch_ring_t<T, false, EPI>(a, pdl, stream);
 }
 
 }  // namespace
 
 int launch_ring(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                bool pdl, cudaStream_t stream) {
+                bool pdl, cudaStream_t stream, const Epilogue& epi) {
   if (M < 1 || M > 4 || N % 8 || K % kGroup) return B200AWQ_ERR_SHAPE;
   const int nsm = sm_count();
   if (nsm == 0) return B200AWQ_ERR_DEVICE;
@@ -390,6 +403,7 @@ int launch_ring(const void* x, const void* qw, const void* sc, const void* sz, v
   const int G = K / kGroup, O = N / 8;
   RingArgs a{};
   a.x = x, a.qw = static_cast<const uint16_t*>(qw), a.sc = sc, a.sz = sz, a.y = y;
+  a.bias = epi.bias, a.residual = epi.residual;
   a.M = M, a.N = N, a.K = K;
   a.S = (G >= 2 * kRingCons && nsm % 2 == 0) ? 2 : 1;
   a.units = nsm / a.S;
@@ -414,10 +428,9 @@ int launch_ring(const void* x, const void* qw, const void* sc, const void* sz, v
   if (ns < 3) return B200AWQ_ERR_SHAPE;  // activations too large next to a useful ring: the caller falls back
   a.NS = ns;
   L.total = off + ns * kSlotBytes;
-  const bool m1 = (M == 1);
   if (dtype == B200AWQ_DTYPE_F16)
-    return m1 ? launch_ring_t<__half, true>(a, pdl, stream) : launch_ring_t<__half, false>(a, pdl, stream);
-  return m1 ? launch_ring_t<__nv_bfloat16, true>(a, pdl, stream) : launch_ring_t<__nv_bfloat16, false>(a, pdl, stream);
+    return epi.on() ? launch_ring_m<__half, true>(a, pdl, stream) : launch_ring_m<__half, false>(a, pdl, stream);
+  return epi.on() ? launch_ring_m<__nv_bfloat16, true>(a, pdl, stream) : launch_ring_m<__nv_bfloat16, false>(a, pdl, stream);
 }
 
 }  // namespace b200awq

@@ -81,11 +81,13 @@ inline StreamSmem stream_smem_layout(int RO, int TT, int MODE, int M, int Kc, bo
 
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
-template <typename T, int RO, int TT>
+// EPI: bias / residual (either may be null) are added to each stored value (add_epilogue); never with the all-reduce
+template <typename T, int RO, int TT, bool EPI>
 __global__ void __launch_bounds__(kStreamWarps * 32, TT == 1 ? 4 : 2)
 w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, const T* __restrict__ scales,
                     const T* __restrict__ szeros, T* __restrict__ y, int M, int N, int K, int Kc, int S,
-                    const __grid_constant__ StreamSmem L, const __grid_constant__ PeerArgs pa) {
+                    const __grid_constant__ StreamSmem L, const __grid_constant__ PeerArgs pa, const T* __restrict__ bias,
+                    const T* __restrict__ residual) {
   constexpr int MODE = TypeTraits<T>::kIsBf16 ? 0 : 2;  // see the header comment
   constexpr int R = 8 * RO;  // output channels per CTA
   constexpr int kStreamThreads = kStreamWarps * 32;
@@ -327,6 +329,7 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
       const int t = e >> 7, row = (e >> 3) & 15, tok = 8 * t + (e & 7);
       if (tok < M && row < R) {
         if (pa.world > 1) cpart[e] = v;  // exchanged with the peer GPUs below
+        else if (EPI) y[(size_t)tok * N + n0 + row] = add_epilogue<T>(from_float<T>(v), bias, residual, (size_t)(n0 + row), (size_t)tok * N + n0 + row);
         else y[(size_t)tok * N + n0 + row] = from_float<T>(v);
       }
     } else {
@@ -353,6 +356,7 @@ w4a16_stream_kernel(const T* __restrict__ x, const uint16_t* __restrict__ qw, co
           float v = cpart[e];
           for (int r = 1; r < S; ++r) v += rbuf[r * TT * 128 + e];  // fixed order
           if (pa.world > 1) cpart[e] = v;  // only this thread reads / writes the leader's own cpart[e]
+          else if (EPI) y[(size_t)tok * N + n0 + row] = add_epilogue<T>(from_float<T>(v), bias, residual, (size_t)(n0 + row), (size_t)tok * N + n0 + row);
           else y[(size_t)tok * N + n0 + row] = from_float<T>(v);
         }
       }
@@ -433,17 +437,17 @@ static int pick_splits(int K, int kc_target) {
 
 // One row block of 8 RO channels per CTA: several per CTA (prefetched up front, activations staged once) would make
 // fat long-lived CTAs that keep the NEXT launch's CTAs from becoming resident, which costs more than the saved prologues.
-template <typename T, int RO, int TT>
+template <typename T, int RO, int TT, bool EPI>
 static int launch_stream_t(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K,
-                           int S, bool pdl, cudaStream_t stream, const PeerArgs* peers) {
+                           int S, bool pdl, cudaStream_t stream, const PeerArgs* peers, const Epilogue& epi) {
   constexpr int MODE = TypeTraits<T>::kIsBf16 ? 0 : 2;
   const int Kc = K / S;
   PeerArgs pa{};
   if (peers) pa = *peers;
-  if (pa.world > 1 && TT != 1) return B200AWQ_ERR_SHAPE;
+  if (pa.world > 1 && (TT != 1 || EPI)) return B200AWQ_ERR_SHAPE;
   const StreamSmem L = stream_smem_layout(RO, TT, MODE, M, Kc, S > 1);
   if (L.total > kStreamSmemCap) return B200AWQ_ERR_SHAPE;
-  if (cudaError_t ea = ensure_dyn_smem<w4a16_stream_kernel<T, RO, TT>>(kStreamSmemCap)) return (int)ea;
+  if (cudaError_t ea = ensure_dyn_smem<w4a16_stream_kernel<T, RO, TT, EPI>>(kStreamSmemCap)) return (int)ea;
   const int ctas = N / (8 * RO) * S;
   // Co-residency: a launch that fits in one wave runs fastest with FEW CTAs per SM (the next launch's
   // CTAs only need enough room to prefetch); multi-wave launches want as many as fit (measured, DESIGN.md).
@@ -453,31 +457,38 @@ static int launch_stream_t(const void* x, const void* qw, const void* sc, const 
   const int per_sm = ctas <= 2 * nsm ? 2 : (ctas <= 3 * nsm ? 3 : 0);
   if (per_sm > 0 && S == 1) dyn = std::max(dyn, (size_t)(233472 / (per_sm + 1) - 512));
   if (dyn > (size_t)kStreamSmemCap) dyn = L.total;
-  return launch_kernel(w4a16_stream_kernel<T, RO, TT>, dim3((unsigned)ctas), dim3(kStreamWarps * 32), dyn, stream, pdl,
-                       (unsigned)S, x, qw, sc, sz, y, M, N, K, Kc, S, L, pa);
+  return launch_kernel(w4a16_stream_kernel<T, RO, TT, EPI>, dim3((unsigned)ctas), dim3(kStreamWarps * 32), dyn, stream, pdl,
+                       (unsigned)S, x, qw, sc, sz, y, M, N, K, Kc, S, L, pa, epi.bias, epi.residual);
+}
+
+template <typename T, bool EPI>
+static int launch_stream_m(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K,
+                           int S, int ro, bool pdl, cudaStream_t stream, const PeerArgs* peers, const Epilogue& epi) {
+  if (M <= 8) {
+    if (ro == 2) return launch_stream_t<T, 2, 1, EPI>(x, qw, sc, sz, y, M, N, K, S, pdl, stream, peers, epi);
+    return launch_stream_t<T, 1, 1, EPI>(x, qw, sc, sz, y, M, N, K, S, pdl, stream, peers, epi);
+  }
+  if (ro == 2) return launch_stream_t<T, 2, 2, EPI>(x, qw, sc, sz, y, M, N, K, S, pdl, stream, peers, epi);
+  return launch_stream_t<T, 1, 2, EPI>(x, qw, sc, sz, y, M, N, K, S, pdl, stream, peers, epi);
 }
 
 template <typename T>
-static int launch_stream_m(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K,
-                           int S, int ro, bool pdl, cudaStream_t stream, const PeerArgs* peers) {
-  if (M <= 8) {
-    if (ro == 2) return launch_stream_t<T, 2, 1>(x, qw, sc, sz, y, M, N, K, S, pdl, stream, peers);
-    return launch_stream_t<T, 1, 1>(x, qw, sc, sz, y, M, N, K, S, pdl, stream, peers);
-  }
-  if (ro == 2) return launch_stream_t<T, 2, 2>(x, qw, sc, sz, y, M, N, K, S, pdl, stream, peers);
-  return launch_stream_t<T, 1, 2>(x, qw, sc, sz, y, M, N, K, S, pdl, stream, peers);
+static int launch_stream_e(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K,
+                           int S, int ro, bool pdl, cudaStream_t stream, const PeerArgs* peers, const Epilogue& epi) {
+  if (epi.on()) return launch_stream_m<T, true>(x, qw, sc, sz, y, M, N, K, S, ro, pdl, stream, peers, epi);
+  return launch_stream_m<T, false>(x, qw, sc, sz, y, M, N, K, S, ro, pdl, stream, peers, epi);
 }
 
 int launch_stream(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                  bool pdl, cudaStream_t stream, const PeerArgs* peers) {
+                  bool pdl, cudaStream_t stream, const PeerArgs* peers, const Epilogue& epi) {
   if (M < 1 || M > 16 || N % 8 || K % kGroup) return B200AWQ_ERR_SHAPE;
   const int ro = (N % 16 == 0) ? 2 : 1;
   // k per CTA: splitting k over a cluster doubles the CTAs and adds the cluster reduction; up to 4 tokens the unsplit
   // 4096 rather than 2048, above that shared memory for x decides
   const int kc_target = M <= 4 ? 4096 : (M <= 8 ? 2048 : 1024);
   const int S = pick_splits(K, kc_target);
-  if (dtype == B200AWQ_DTYPE_F16) return launch_stream_m<__half>(x, qw, sc, sz, y, M, N, K, S, ro, pdl, stream, peers);
-  return launch_stream_m<__nv_bfloat16>(x, qw, sc, sz, y, M, N, K, S, ro, pdl, stream, peers);
+  if (dtype == B200AWQ_DTYPE_F16) return launch_stream_e<__half>(x, qw, sc, sz, y, M, N, K, S, ro, pdl, stream, peers, epi);
+  return launch_stream_e<__nv_bfloat16>(x, qw, sc, sz, y, M, N, K, S, ro, pdl, stream, peers, epi);
 }
 
 }  // namespace b200awq

@@ -148,6 +148,36 @@ __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity
   } while (!ok);
 }
 
+// add_epilogue over the 8 consecutive elements of one 16-byte store of y, given the matching 16 B of the bias (b, if
+// has_bias) and of the residual (r, if has_res).  Works on the 16-bit halves of 32-bit words (no local arrays).
+template <typename T>
+__device__ __forceinline__ uint4 add_epilogue_x8(uint4 v, bool has_bias, uint4 b, bool has_res, uint4 r) {
+  auto f = [](uint32_t w, int h) {  // element h of word w as fp32
+    const unsigned short b = (unsigned short)(w >> (16 * h));
+    if constexpr (TypeTraits<T>::kIsBf16) return __bfloat162float(__ushort_as_bfloat16(b));
+    else return __half2float(__ushort_as_half(b));
+  };
+  auto bits = [](float x) -> uint32_t {
+    if constexpr (TypeTraits<T>::kIsBf16) return __bfloat16_as_ushort(from_float<T>(x));
+    else return __half_as_ushort(from_float<T>(x));
+  };
+  uint32_t vw[4] = {v.x, v.y, v.z, v.w};
+  const uint32_t bw[4] = {b.x, b.y, b.z, b.w}, rw[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    uint32_t o = 0;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {  // add_epilogue, element by element
+      uint32_t e = (vw[q] >> (16 * h)) & 0xffffu;
+      if (has_bias) e = bits(f(e, 0) + f(bw[q], h));
+      if (has_res) e = bits(f(rw[q], h) + f(e, 0));
+      o |= e << (16 * h);
+    }
+    vw[q] = o;
+  }
+  return make_uint4(vw[0], vw[1], vw[2], vw[3]);
+}
+
 template <int TN>
 struct WgSmem {
   static constexpr int kXBytes = TN * 128;  // TN token rows x 64 k x 2 B (a multiple of 1024: stages stay aligned)
@@ -160,10 +190,13 @@ struct WgSmem {
   static constexpr int kTotal = kStages * kStageBytes + kEpiBytes + 1024 /*align*/ + 256 /*barriers*/;
 };
 
-template <typename T, int TN>
+// EPI: bias / residual (either may be null) are added to each stored value (add_epilogue).  TN stays the last template
+// argument: tests read the token tile from the end of the kernel's name.
+template <typename T, bool EPI, int TN>
 __global__ void __launch_bounds__(kWgThreads, 1)
 w4a16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w,
-                   const T* __restrict__ scales, const T* __restrict__ szeros, T* __restrict__ y, int M, int N, int K, int S) {
+                   const T* __restrict__ scales, const T* __restrict__ szeros, T* __restrict__ y, int M, int N, int K, int S,
+                   const T* __restrict__ bias, const T* __restrict__ residual) {
   using L = WgSmem<TN>;
   constexpr int STAGES = L::kStages;
   constexpr int NA = TN / 2;  // accumulator registers per thread
@@ -283,6 +316,9 @@ w4a16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_consta
 
       // ------------------------------------------------ epilogue for this tile
       // acc[4 i + e]: channel r0 + 8 (e >> 1), token 8 i + 2 t + (e & 1)
+      // The consumers already follow the producer's griddepcontrol.wait (through the full barriers); their own wait
+      // makes the stream order of bias / residual explicit and returns at once.
+      if (EPI) pdl_wait_prior_grid();
       if (S > 1) {
         // split-K: fp32 partial tile -> own shared memory; every rank then reduces TN / S tokens of the tile over
         // distributed shared memory and stores them (no atomics, fixed summation order)
@@ -302,7 +338,8 @@ w4a16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_consta
           if (tt < TN && tok < M) {
             float v = 0.f;
             for (int r = 0; r < S; ++r) v += ld_cluster_f32(map_to_rank(base + (uint32_t)(tt * kBM + ch) * 4u, (uint32_t)r));
-            y[(size_t)tok * N + oc_tile * kBM + ch] = from_float<T>(v);
+            const size_t i = (size_t)tok * N + oc_tile * kBM + ch;
+            y[i] = EPI ? add_epilogue<T>(from_float<T>(v), bias, residual, (size_t)(oc_tile * kBM + ch), i) : from_float<T>(v);
           }
         }
         __syncwarp();
@@ -315,13 +352,39 @@ w4a16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_consta
           const int tok = 8 * (i >> 2) + 2 * t + (i & 1), ch = r0 + 8 * ((i >> 1) & 1);
           *reinterpret_cast<T*>(epi + tok * L::kOutRow + ch * 2) = from_float<T>(acc[i]);
         }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        for (int e = ct; e < TN * 16; e += 256) {
-          const int rr = e >> 4, cc = e & 15;
-          const int tok = tok_tile * TN + rr;
-          if (tok < M)
-            *reinterpret_cast<uint4*>(y + (size_t)tok * N + oc_tile * kBM + cc * 8) =
-                *reinterpret_cast<const uint4*>(epi + rr * L::kOutRow + cc * 16);
+        if constexpr (EPI) {
+          // the 16-byte stores below, thread ct taking pieces ct + 256 p: always the same 8 channels (one bias load),
+          // TN / 16 token rows.  Bias and residual are loaded BEFORE the barrier, so that their latency overlaps the
+          // wait for the other warps' staging.
+          constexpr int kPieces = TN / 16;
+          const int cc = ct & 15;
+          const size_t n = (size_t)oc_tile * kBM + cc * 8;
+          const uint4 zero = make_uint4(0, 0, 0, 0);
+          const uint4 bv = bias ? *reinterpret_cast<const uint4*>(bias + n) : zero;
+          uint4 rv[kPieces];
+#pragma unroll
+          for (int p = 0; p < kPieces; ++p) {
+            const int tok = tok_tile * TN + (ct >> 4) + 16 * p;
+            rv[p] = residual && tok < M ? *reinterpret_cast<const uint4*>(residual + (size_t)tok * N + n) : zero;
+          }
+          asm volatile("bar.sync 1, 256;" ::: "memory");
+#pragma unroll
+          for (int p = 0; p < kPieces; ++p) {
+            const int rr = (ct >> 4) + 16 * p, tok = tok_tile * TN + rr;
+            if (tok < M) {
+              const uint4 v = *reinterpret_cast<const uint4*>(epi + rr * L::kOutRow + cc * 16);
+              *reinterpret_cast<uint4*>(y + (size_t)tok * N + n) = add_epilogue_x8<T>(v, bias, bv, residual, rv[p]);
+            }
+          }
+        } else {
+          asm volatile("bar.sync 1, 256;" ::: "memory");
+          for (int e = ct; e < TN * 16; e += 256) {
+            const int rr = e >> 4, cc = e & 15;
+            const int tok = tok_tile * TN + rr;
+            if (tok < M)
+              *reinterpret_cast<uint4*>(y + (size_t)tok * N + oc_tile * kBM + cc * 8) =
+                  *reinterpret_cast<const uint4*>(epi + rr * L::kOutRow + cc * 16);
+          }
         }
         asm volatile("bar.sync 1, 256;" ::: "memory");  // staging buffer free for the next tile
       }
@@ -335,9 +398,9 @@ w4a16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_consta
 
 // ------------------------------------------------------------------------------------ host
 // max_clusters <= 0: one cluster per tile (all resident at once when they fit); else a persistent grid of that many
-template <typename T, int TN>
+template <typename T, int TN, bool EPI>
 static int launch_wgmma_t(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K,
-                          bool pdl, int max_clusters, int S, cudaStream_t stream) {
+                          bool pdl, int max_clusters, int S, const Epilogue& epi, cudaStream_t stream) {
   using L = WgSmem<TN>;
   EncodeTiledFn enc = get_encoder();
   if (!enc) return B200AWQ_ERR_DRIVER;
@@ -362,33 +425,37 @@ static int launch_wgmma_t(const void* x, const void* qw, const void* sc, const v
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return B200AWQ_ERR_DRIVER;
   }
-  if (cudaError_t ea = ensure_dyn_smem<w4a16_wgmma_kernel<T, TN>>(L::kTotal)) return (int)ea;
+  if (cudaError_t ea = ensure_dyn_smem<w4a16_wgmma_kernel<T, EPI, TN>>(L::kTotal)) return (int)ea;
   const int tiles = ((M + TN - 1) / TN) * (N / kBM);
   int clusters = tiles;
   if (max_clusters > 0 && max_clusters < clusters) clusters = max_clusters;
-  return launch_kernel(w4a16_wgmma_kernel<T, TN>, dim3((unsigned)(clusters * S)), dim3(kWgThreads), (size_t)L::kTotal, stream,
-                       pdl, (unsigned)S, tm_x, tm_w, sc, sz, y, M, N, K, S);
+  return launch_kernel(w4a16_wgmma_kernel<T, EPI, TN>, dim3((unsigned)(clusters * S)), dim3(kWgThreads), (size_t)L::kTotal,
+                       stream, pdl, (unsigned)S, tm_x, tm_w, sc, sz, y, M, N, K, S, epi.bias, epi.residual);
 }
 
-template <typename T>
+template <typename T, bool EPI>
 static int launch_wgmma_tn(int tn, const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N,
-                           int K, bool pdl, int max_clusters, int S, cudaStream_t stream) {
+                           int K, bool pdl, int max_clusters, int S, const Epilogue& epi, cudaStream_t stream) {
   switch (tn) {
-    case 16: return launch_wgmma_t<T, 16>(x, qw, sc, sz, y, M, N, K, pdl, max_clusters, S, stream);
-    case 32: return launch_wgmma_t<T, 32>(x, qw, sc, sz, y, M, N, K, pdl, max_clusters, S, stream);
-    case 64: return launch_wgmma_t<T, 64>(x, qw, sc, sz, y, M, N, K, pdl, max_clusters, S, stream);
-    default: return launch_wgmma_t<T, 128>(x, qw, sc, sz, y, M, N, K, pdl, max_clusters, S, stream);
+    case 16: return launch_wgmma_t<T, 16, EPI>(x, qw, sc, sz, y, M, N, K, pdl, max_clusters, S, epi, stream);
+    case 32: return launch_wgmma_t<T, 32, EPI>(x, qw, sc, sz, y, M, N, K, pdl, max_clusters, S, epi, stream);
+    case 64: return launch_wgmma_t<T, 64, EPI>(x, qw, sc, sz, y, M, N, K, pdl, max_clusters, S, epi, stream);
+    default: return launch_wgmma_t<T, 128, EPI>(x, qw, sc, sz, y, M, N, K, pdl, max_clusters, S, epi, stream);
   }
 }
 
 static int launch_wgmma(int tn, const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K,
-                        int dtype, bool pdl, int max_clusters, int S, cudaStream_t stream) {
-  if (dtype == B200AWQ_DTYPE_F16) return launch_wgmma_tn<__half>(tn, x, qw, sc, sz, y, M, N, K, pdl, max_clusters, S, stream);
-  return launch_wgmma_tn<__nv_bfloat16>(tn, x, qw, sc, sz, y, M, N, K, pdl, max_clusters, S, stream);
+                        int dtype, bool pdl, int max_clusters, int S, const Epilogue& epi, cudaStream_t stream) {
+  const bool f16 = dtype == B200AWQ_DTYPE_F16;
+  if (epi.on())
+    return f16 ? launch_wgmma_tn<__half, true>(tn, x, qw, sc, sz, y, M, N, K, pdl, max_clusters, S, epi, stream)
+               : launch_wgmma_tn<__nv_bfloat16, true>(tn, x, qw, sc, sz, y, M, N, K, pdl, max_clusters, S, epi, stream);
+  return f16 ? launch_wgmma_tn<__half, false>(tn, x, qw, sc, sz, y, M, N, K, pdl, max_clusters, S, epi, stream)
+             : launch_wgmma_tn<__nv_bfloat16, false>(tn, x, qw, sc, sz, y, M, N, K, pdl, max_clusters, S, epi, stream);
 }
 
 int launch_umma(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                bool pdl, cudaStream_t stream) {
+                bool pdl, cudaStream_t stream, const Epilogue& epi) {
   if (M < 1 || N % kBM || K % kGroup) return B200AWQ_ERR_SHAPE;
   const int sms = sm_count();
   if (sms == 0) return B200AWQ_ERR_DEVICE;
@@ -410,14 +477,14 @@ int launch_umma(const void* x, const void* qw, const void* sc, const void* sz, v
     }
   }
   // a persistent grid of one CTA per SM
-  return launch_wgmma(tn, x, qw, sc, sz, y, M, N, K, dtype, pdl, sms / S > 0 ? sms / S : 1, S, stream);
+  return launch_wgmma(tn, x, qw, sc, sz, y, M, N, K, dtype, pdl, sms / S > 0 ? sms / S : 1, S, epi, stream);
 }
 
 // Skinny batches (HBM-bound): one 16-token tile, one CTA per 128 output channels and k slice, every CTA resident at
 // once so that several stream their weights per SM.  The k split is the smallest (<= 8, dividing the group count)
 // whose slice is <= 512 k, or <= 1024 k once there are at least two CTAs per SM.
 int launch_flat(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                bool pdl, cudaStream_t stream) {
+                bool pdl, cudaStream_t stream, const Epilogue& epi) {
   if (M < 1 || M > 16 || N % kBM || K % kGroup) return B200AWQ_ERR_SHAPE;
   const int groups = K / kGroup;
   const int sms = sm_count();
@@ -430,7 +497,7 @@ int launch_flat(const void* x, const void* qw, const void* sc, const void* sz, v
     if (kc <= 512) break;
     if (kc <= 1024 && (N / kBM) * s >= 2 * sms) break;
   }
-  return launch_wgmma(16, x, qw, sc, sz, y, M, N, K, dtype, pdl, 0, S, stream);
+  return launch_wgmma(16, x, qw, sc, sz, y, M, N, K, dtype, pdl, 0, S, epi, stream);
 }
 
 }  // namespace b200awq

@@ -31,6 +31,8 @@ def lib() -> ctypes.CDLL:
         L.gemm_forward_4bit.restype = ci
         L.b200awq_w4a16_gemv_allreduce.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp, vp]
         L.b200awq_w4a16_gemv_allreduce.restype = ci
+        L.b200awq_w4a16_linear.argtypes = [vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp]
+        L.b200awq_w4a16_linear.restype = ci
         L.b200awq_w4a16_gemm_workspace_bytes.argtypes = [ci, ci, ci]
         L.b200awq_w4a16_gemm_workspace_bytes.restype = sz
         L.b200awq_w4a16_mlp_front.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp, sz, vp]

@@ -133,9 +133,14 @@ class WQLinear(nn.Module):
         return awq_linear
 
     @torch.no_grad()
-    def forward(self, x):
+    def forward(self, x, residual=None):
+        """x W~^T (+ bias) (+ residual).  With a bias or a residual, one launch adds them in the kernel's epilogue,
+        bit-identical to the reference's `out + self.bias` and the decoder block's `residual + out`."""
         eng = _get_engine()
         inputs = x if x.is_contiguous() else x.contiguous()
+        if self.bias is not None or residual is not None:
+            return eng.w4a16_linear_forward_cuda(inputs, self.qweight, self.scales, self.scaled_zeros, self.group_size,
+                                                 bias=self.bias, residual=residual)
         m = inputs.numel() // inputs.shape[-1]
         if inputs.numel() / inputs.shape[-1] < 8:  # reference dispatch rule, qmodule.py:206
             out = eng.gemv_forward_cuda_new(inputs, self.qweight, self.scales, self.scaled_zeros,
