@@ -47,7 +47,7 @@ bool pdl_enabled() { return g_pdl.load(std::memory_order_relaxed); }
 using b200awq::aligned16;
 
 // `r` passed through; a successful entry that launched a kernel counts one launch (b200awq_launch_count)
-int counted(int r, bool launched) {
+int counted(int r, bool launched = true) {
   if (r == 0 && launched) g_launches.fetch_add(1, std::memory_order_relaxed);
   return r;
 }
@@ -109,33 +109,66 @@ bool use_flat(int m, int n, int k) {
   return n % 128 == 0 && m >= min_m && m <= kFlatMaxM;
 }
 
-// Small token counts (decode and the bottom of the batch sweep): decode (one token) -> ring -> flat -> stream, each returning
-// B200AWQ_ERR_SHAPE (or, for the cluster kernels, a launch-configuration error) when it cannot take the shape.
-int launch_small(const void* x, const void* qw, const void* sc, const void* sz, void* y, int m, int n, int k, int dtype,
-                 cudaStream_t st, const b200awq::Epilogue& epi = {}) {
+// One W4A16 product y = x W~^T (+ epilogue), as validated by the entry.
+struct W4Operands {
+  const void *x, *qw, *sc, *sz;
+  void* y;
+  int m, n, k, dtype;
+  cudaStream_t st;
+  b200awq::Epilogue epi;
+};
+
+// The kernels an entry may route to.
+enum class Envelope {
+  kGemv,           // the small-token kernels only (b200awq_w4a16_gemv; b200awq_w4a16_linear below 8 tokens)
+  kGemm,           // the small-token kernels, else the wgmma tile kernel (b200awq_w4a16_gemm; linear from 8 tokens)
+  kMlpProjection,  // as kGemm, but without kGemm's 9..16-token big-layer rule (each of mlp_front's two projections)
+};
+
+// Routing of every W4A16 entry.  Small token counts take decode (one fp16 token) -> ring -> flat -> stream, each returning
+// B200AWQ_ERR_SHAPE (or, for the cluster kernels, a launch-configuration error) when it cannot take the shape; outside
+// kGemv, a shape none of them takes goes to the 128-channel wgmma tiles (split-k over a cluster for small token counts).
+int launch_w4a16(const W4Operands& o, Envelope env) {
+  const auto& [x, qw, sc, sz, y, m, n, k, dtype, st, epi] = o;
+  const bool pdl = pdl_enabled();
+  // kGemm: 9..16 tokens on the large layers (>= 48 M weights) take the persistent tile launch (split-k) directly
+  const bool big_mid = env == Envelope::kGemm && m > 8 && (long long)n * k >= 48ll * 1000 * 1000;
   int r = B200AWQ_ERR_SHAPE;
-  if (use_decode(m, dtype))
-    r = next_on_config_error(b200awq::launch_decode(x, qw, sc, sz, y, n, k, dtype, pdl_enabled(), decode_tuning(), st, epi));
-  if (r != 0 && m <= kRingMaxM)
-    r = next_on_config_error(b200awq::launch_ring(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st, epi));
-  if (r != 0 && use_flat(m, n, k))
-    r = next_on_config_error(b200awq::launch_flat(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st, epi));
-  if (r != 0 && m <= kStreamMaxM) r = b200awq::launch_stream(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st, nullptr, epi);
+  if (!big_mid) {
+    if (use_decode(m, dtype))
+      r = next_on_config_error(b200awq::launch_decode(x, qw, sc, sz, y, n, k, dtype, pdl, decode_tuning(), st, epi));
+    if (r != 0 && m <= kRingMaxM) r = next_on_config_error(b200awq::launch_ring(x, qw, sc, sz, y, m, n, k, dtype, pdl, st, epi));
+    if (r != 0 && use_flat(m, n, k)) r = next_on_config_error(b200awq::launch_flat(x, qw, sc, sz, y, m, n, k, dtype, pdl, st, epi));
+    if (r != 0 && m <= kStreamMaxM) r = b200awq::launch_stream(x, qw, sc, sz, y, m, n, k, dtype, pdl, st, nullptr, epi);
+  }
+  if (env != Envelope::kGemv && r == B200AWQ_ERR_SHAPE && n % 128 == 0)
+    r = b200awq::launch_umma(x, qw, sc, sz, y, m, n, k, dtype, pdl, st, epi);
   return r;
 }
 
-// Routing of b200awq_w4a16_gemm (and of b200awq_w4a16_linear from 8 tokens): the small-token kernels, else the wgmma tile
-// kernel.  n % 128 == 0.
-int launch_gemm(const void* x, const void* qw, const void* sc, const void* sz, void* y, int m, int n, int k, int dtype,
-                cudaStream_t st, const b200awq::Epilogue& epi = {}) {
-  int r = B200AWQ_ERR_SHAPE;
-  // 9..16 tokens on the large layers (>= 48 M weights): the persistent tile launch (split-k); everything else below
-  // 17 tokens: the small-token kernels
-  const bool big_mid = m > 8 && (long long)n * k >= 48ll * 1000 * 1000;
-  if (m <= 16 && !big_mid) r = launch_small(x, qw, sc, sz, y, m, n, k, dtype, st, epi);
-  if (r == B200AWQ_ERR_SHAPE)  // 128-channel wgmma tiles; split-k over a cluster for small token counts
-    r = b200awq::launch_umma(x, qw, sc, sz, y, m, n, k, dtype, pdl_enabled(), st, epi);
-  return r;
+// The TMA attention entries' common checks: dtype, sizes, head ratio and scale (the softmax runs on the raw scores'
+// max: scale > 0).  kv_heads >= 1 once this passes.
+int check_attention(int dtype, int batch, int seqlen_q, int seqlen_k, int heads, int kv_heads, float softmax_scale) {
+  if (int e = check_dtype(dtype)) return e;
+  if (batch < 0 || seqlen_q < 0 || seqlen_k < 0 || heads < 1 || kv_heads < 1 || heads % kv_heads ||
+      !(std::isfinite(softmax_scale) && softmax_scale > 0.f))
+    return B200AWQ_ERR_SHAPE;
+  return 0;
+}
+
+// q, k, v, out and the strides of the operands read through TMA (16-byte multiples; Q is read in 16-byte pieces)
+int check_attention_operands(const void* q, const void* k, const void* v, const void* out,
+                             std::initializer_list<const long long*> strides) {
+  if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(out)) return B200AWQ_ERR_ALIGN;
+  for (const long long* s : strides)
+    if (!s || s[0] % 8 || s[1] % 8 || s[2] % 8) return B200AWQ_ERR_ALIGN;
+  return 0;
+}
+
+int check_workspace(const void* workspace, size_t workspace_bytes, size_t need) {
+  if (workspace && !aligned16(workspace)) return B200AWQ_ERR_ALIGN;
+  if (workspace_bytes < need || (workspace_bytes && !workspace)) return B200AWQ_ERR_WORKSPACE;
+  return 0;
 }
 
 }  // namespace
@@ -146,7 +179,8 @@ int b200awq_w4a16_gemv(const void* x, const void* qweight, const void* scales, c
                        int k, int group_size, int dtype, void* stream) {
   if (int e = check_common(x, qweight, scales, szeros, y, m, n, k, group_size, dtype)) return e;
   if (m > 7) return B200AWQ_ERR_BATCH;  // reference envelope: gemv_cuda.cu:291-330
-  return counted(launch_small(x, qweight, scales, szeros, y, m, n, k, dtype, static_cast<cudaStream_t>(stream)), true);
+  const W4Operands o{x, qweight, scales, szeros, y, m, n, k, dtype, static_cast<cudaStream_t>(stream)};
+  return counted(launch_w4a16(o, Envelope::kGemv));
 }
 
 int b200awq_w4a16_linear(const void* x, const void* qweight, const void* scales, const void* szeros, const void* bias,
@@ -155,12 +189,9 @@ int b200awq_w4a16_linear(const void* x, const void* qweight, const void* scales,
   if ((bias && !aligned16(bias)) || (residual && !aligned16(residual))) return B200AWQ_ERR_ALIGN;
   if (m >= 8 && n % 128) return B200AWQ_ERR_SHAPE;  // the GEMM envelope (b200awq_w4a16_gemm)
   if (int e = check_device()) return e;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const b200awq::Epilogue epi{bias, residual};
+  const W4Operands o{x, qweight, scales, szeros, y, m, n, k, dtype, static_cast<cudaStream_t>(stream), {bias, residual}};
   // the reference's dispatch rule (awq/quantize/qmodule.py:206): the GEMV's routes below 8 tokens, the GEMM's from 8
-  return counted(m < 8 ? launch_small(x, qweight, scales, szeros, y, m, n, k, dtype, st, epi)
-                       : launch_gemm(x, qweight, scales, szeros, y, m, n, k, dtype, st, epi),
-                 true);
+  return counted(launch_w4a16(o, m < 8 ? Envelope::kGemv : Envelope::kGemm));
 }
 
 int b200awq_w4a16_gemv_allreduce(const void* x, const void* qweight, const void* scales, const void* szeros, void* y, int m,
@@ -181,8 +212,7 @@ int b200awq_w4a16_gemv_allreduce(const void* x, const void* qweight, const void*
   pa.tok_cap = peers->cap_words / peers->n_max;
   pa.cap = pa.tok_cap * peers->n_max;
   return counted(b200awq::launch_stream(x, qweight, scales, szeros, y, m, n, k, dtype, pdl_enabled(),
-                                        static_cast<cudaStream_t>(stream), &pa),
-                 true);
+                                        static_cast<cudaStream_t>(stream), &pa));
 }
 
 size_t b200awq_w4a16_mlp_front_workspace_bytes(int m, int n, int) { return m > 0 && n > 0 ? (size_t)2 * m * n * 2 : 0; }
@@ -198,21 +228,16 @@ int b200awq_w4a16_mlp_front(const void* x, const void* gate_qweight, const void*
   if (use_decode(m, dtype) &&
       next_on_config_error(b200awq::launch_decode_mlp_front(x, gate_qweight, gate_scales, gate_szeros, up_qweight, up_scales,
                                                             up_szeros, y, n, k, dtype, pdl_enabled(), decode_tuning(), st)) == 0)
-    return counted(0, true);
+    return counted(0);
   const size_t half = (size_t)m * n * 2;
   if (!workspace || workspace_bytes < 2 * half || !aligned16(workspace)) return B200AWQ_ERR_WORKSPACE;
   void* g = workspace;
   void* u = static_cast<char*>(workspace) + half;
-  for (int t = 0; t < 2; ++t) {
-    const void* qw = t ? up_qweight : gate_qweight;
-    const void* sc = t ? up_scales : gate_scales;
-    const void* sz = t ? up_szeros : gate_szeros;
-    int r = B200AWQ_ERR_SHAPE;
-    if (m <= 16) r = launch_small(x, qw, sc, sz, t ? u : g, m, n, k, dtype, st);
-    if (r == B200AWQ_ERR_SHAPE && n % 128 == 0) r = b200awq::launch_umma(x, qw, sc, sz, t ? u : g, m, n, k, dtype, pdl_enabled(), st);
-    if (counted(r, true) != 0) return r;
-  }
-  return counted(b200awq::launch_silu_mul(g, u, y, 1, (size_t)m * n, (size_t)m * n, dtype, pdl_enabled(), st), true);
+  const W4Operands gate{x, gate_qweight, gate_scales, gate_szeros, g, m, n, k, dtype, st};
+  const W4Operands up{x, up_qweight, up_scales, up_szeros, u, m, n, k, dtype, st};
+  for (const W4Operands* o : {&gate, &up})
+    if (int r = counted(launch_w4a16(*o, Envelope::kMlpProjection))) return r;
+  return counted(b200awq::launch_silu_mul(g, u, y, 1, (size_t)m * n, (size_t)m * n, dtype, pdl_enabled(), st));
 }
 
 size_t b200awq_single_query_attention_workspace_bytes(int batch, int heads, int kv_heads, int head_dim, int max_len) {
@@ -231,30 +256,22 @@ int b200awq_single_query_attention(const void* q, const void* k, const void* v, 
   return counted(b200awq::launch_single_query_attention(q, k, v, k_cache, v_cache, out, length_per_sample, batch, heads, kv_heads,
                                                         head_dim, max_len, timestep, q_batch_stride, k_batch_stride, v_batch_stride,
                                                         rotary_dim, rotary_base, rotary_scale, neox, dtype, workspace,
-                                                        workspace_bytes, pdl_enabled(), static_cast<cudaStream_t>(stream)),
-                 true);
+                                                        workspace_bytes, pdl_enabled(), static_cast<cudaStream_t>(stream)));
 }
 
 int b200awq_prefill_attention(const void* q, const void* k, const void* v, void* out, const int* cu_seqlens_q,
                               const int* cu_seqlens_k, int batch, int seqlen_q, int seqlen_k, int heads, int kv_heads,
                               int head_dim, const long long q_strides[3], const long long k_strides[3],
                               const long long v_strides[3], float softmax_scale, int causal, int dtype, void* stream) {
-  if (int e = check_dtype(dtype)) return e;
-  if (batch < 0 || seqlen_q < 0 || seqlen_k < 0 || heads < 1 || kv_heads < 1 || heads % kv_heads ||
-      (head_dim != 64 && head_dim != 72 && head_dim != 128) || !(std::isfinite(softmax_scale) && softmax_scale > 0.f))
-    return B200AWQ_ERR_SHAPE;  // the softmax runs on the raw scores' max: scale > 0
-  if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(out) || !q_strides || !k_strides || !v_strides)
-    return B200AWQ_ERR_ALIGN;
+  if (int e = check_attention(dtype, batch, seqlen_q, seqlen_k, heads, kv_heads, softmax_scale)) return e;
+  if (head_dim != 64 && head_dim != 72 && head_dim != 128) return B200AWQ_ERR_SHAPE;
+  if (int e = check_attention_operands(q, k, v, out, {q_strides, k_strides, v_strides})) return e;
   if ((cu_seqlens_q == nullptr) != (cu_seqlens_k == nullptr)) return B200AWQ_ERR_ALIGN;
-  for (const long long* s : {q_strides, k_strides, v_strides})
-    for (int i = 0; i < 3; ++i)
-      if (s[i] % 8) return B200AWQ_ERR_ALIGN;  // TMA takes 16-byte strides
   if (int e = check_device()) return e;
   if (batch == 0 || seqlen_q == 0) return 0;
   return counted(b200awq::launch_prefill_attention(q, k, v, out, cu_seqlens_q, cu_seqlens_k, batch, seqlen_q, seqlen_k, heads,
                                                    kv_heads, head_dim, q_strides, k_strides, v_strides, softmax_scale, causal != 0,
-                                                   dtype, static_cast<cudaStream_t>(stream)),
-                 true);
+                                                   dtype, static_cast<cudaStream_t>(stream)));
 }
 
 size_t b200awq_splitkv_attention_workspace_bytes(int batch, int seqlen_q, int seqlen_k, int heads, int kv_heads, int head_dim) {
@@ -265,26 +282,17 @@ int b200awq_splitkv_attention(const void* q, const void* k, const void* v, void*
                               int heads, int kv_heads, int head_dim, const long long q_strides[3],
                               const long long k_strides[3], const long long v_strides[3], float softmax_scale, int causal,
                               int dtype, void* workspace, size_t workspace_bytes, void* stream) {
-  if (int e = check_dtype(dtype)) return e;
-  if (batch < 0 || seqlen_q < 0 || seqlen_k < 0 || heads < 1 || kv_heads < 1 || heads % kv_heads ||
-      (long long)seqlen_q * (heads / kv_heads) > 64 || (head_dim != 64 && head_dim != 128) ||
-      !(std::isfinite(softmax_scale) && softmax_scale > 0.f))
-    return B200AWQ_ERR_SHAPE;  // the softmax runs on the raw scores' max: scale > 0
-  if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(out) || !q_strides || !k_strides || !v_strides)
-    return B200AWQ_ERR_ALIGN;
-  for (const long long* s : {q_strides, k_strides, v_strides})
-    for (int i = 0; i < 3; ++i)
-      if (s[i] % 8) return B200AWQ_ERR_ALIGN;  // TMA takes 16-byte strides; Q is read in 16-byte pieces
-  if (workspace && !aligned16(workspace)) return B200AWQ_ERR_ALIGN;
-  if (workspace_bytes < b200awq::splitkv_attention_workspace_bytes(batch, seqlen_q, seqlen_k, heads, kv_heads, head_dim) ||
-      (workspace_bytes && !workspace))
-    return B200AWQ_ERR_WORKSPACE;
+  if (int e = check_attention(dtype, batch, seqlen_q, seqlen_k, heads, kv_heads, softmax_scale)) return e;
+  if ((long long)seqlen_q * (heads / kv_heads) > 64 || (head_dim != 64 && head_dim != 128)) return B200AWQ_ERR_SHAPE;
+  if (int e = check_attention_operands(q, k, v, out, {q_strides, k_strides, v_strides})) return e;
+  if (int e = check_workspace(workspace, workspace_bytes,
+                              b200awq::splitkv_attention_workspace_bytes(batch, seqlen_q, seqlen_k, heads, kv_heads, head_dim)))
+    return e;
   if (int e = check_device()) return e;
   if (batch == 0 || seqlen_q == 0) return 0;
   return counted(b200awq::launch_splitkv_attention(q, k, v, out, batch, seqlen_q, seqlen_k, heads, kv_heads, head_dim, q_strides,
                                                    k_strides, v_strides, softmax_scale, causal != 0, dtype, workspace,
-                                                   workspace_bytes, static_cast<cudaStream_t>(stream)),
-                 true);
+                                                   workspace_bytes, static_cast<cudaStream_t>(stream)));
 }
 
 size_t b200awq_kv_cache_attention_workspace_bytes(int layout, int batch, int seqlen_q, int seqlen_k, int heads,
@@ -296,25 +304,20 @@ int b200awq_kv_cache_attention(const void* q, const void* k_cache, const void* v
                                int seqlen_q, int seqlen_k, int max_len, int heads, int kv_heads, int head_dim,
                                const long long q_strides[3], float softmax_scale, int causal, int dtype, void* workspace,
                                size_t workspace_bytes, void* stream) {
-  if (int e = check_dtype(dtype)) return e;
-  if ((layout != B200AWQ_KV_FT && layout != B200AWQ_KV_BTHD) || batch < 0 || seqlen_q < 0 || seqlen_k < 0 ||
-      max_len < 1 || seqlen_k > max_len || heads < 1 || kv_heads < 1 || heads % kv_heads ||
-      (head_dim != 64 && head_dim != 128) || !(std::isfinite(softmax_scale) && softmax_scale > 0.f))
-    return B200AWQ_ERR_SHAPE;  // the softmax runs on the raw scores' max: scale > 0
-  if (!aligned16(q) || !aligned16(k_cache) || !aligned16(v_cache) || !aligned16(out) || !q_strides) return B200AWQ_ERR_ALIGN;
-  for (int i = 0; i < 3; ++i)
-    if (q_strides[i] % 8) return B200AWQ_ERR_ALIGN;  // Q is read in 16-byte pieces
-  if (workspace && !aligned16(workspace)) return B200AWQ_ERR_ALIGN;
-  if (workspace_bytes < b200awq::kv_cache_attention_workspace_bytes(layout, batch, seqlen_q, seqlen_k, heads, kv_heads,
-                                                                    head_dim) ||
-      (workspace_bytes && !workspace))
-    return B200AWQ_ERR_WORKSPACE;
-  if (batch == 0 || seqlen_q == 0) return 0;
+  if (int e = check_attention(dtype, batch, seqlen_q, seqlen_k, heads, kv_heads, softmax_scale)) return e;
+  if ((layout != B200AWQ_KV_FT && layout != B200AWQ_KV_BTHD) || max_len < 1 || seqlen_k > max_len ||
+      (head_dim != 64 && head_dim != 128))
+    return B200AWQ_ERR_SHAPE;
+  if (int e = check_attention_operands(q, k_cache, v_cache, out, {q_strides})) return e;  // the caches are not strided
+  if (int e = check_workspace(workspace, workspace_bytes,
+                              b200awq::kv_cache_attention_workspace_bytes(layout, batch, seqlen_q, seqlen_k, heads,
+                                                                          kv_heads, head_dim)))
+    return e;
+  if (batch == 0 || seqlen_q == 0) return 0;  // unlike the two entries above, before the device check
   if (int e = check_device()) return e;
   return counted(b200awq::launch_kv_cache_attention(q, k_cache, v_cache, out, layout, batch, seqlen_q, seqlen_k, max_len, heads,
                                                     kv_heads, head_dim, q_strides, softmax_scale, causal != 0, dtype,
-                                                    workspace, workspace_bytes, static_cast<cudaStream_t>(stream)),
-                 true);
+                                                    workspace, workspace_bytes, static_cast<cudaStream_t>(stream)));
 }
 
 int b200awq_rope_with_pos(const void* x, const float* freqs, void* y, int s, int b, int h, int d, int d2,
@@ -323,8 +326,7 @@ int b200awq_rope_with_pos(const void* x, const float* freqs, void* y, int s, int
   if (!x || !freqs || !y || !in_strides || !out_strides) return B200AWQ_ERR_ALIGN;
   if (int e = check_device()) return e;
   return counted(b200awq::launch_rope_with_pos(x, freqs, y, s, b, h, d, d2, in_strides, out_strides, dtype, pdl_enabled(),
-                                               static_cast<cudaStream_t>(stream)),
-                 true);
+                                               static_cast<cudaStream_t>(stream)));
 }
 
 int b200awq_rotary_embedding_neox(const long long* positions, void* query, void* key, const void* cos_sin_cache, int tokens,
@@ -344,7 +346,7 @@ int b200awq_rmsnorm(const void* x, const void* gamma, void* y, int m, int n, flo
   if (!x || !gamma || !y) return B200AWQ_ERR_ALIGN;
   if (int e = check_device()) return e;
   if (m == 0) return 0;
-  return counted(b200awq::launch_rmsnorm(x, gamma, y, eps, m, n, dtype, pdl_enabled(), static_cast<cudaStream_t>(stream)), true);
+  return counted(b200awq::launch_rmsnorm(x, gamma, y, eps, m, n, dtype, pdl_enabled(), static_cast<cudaStream_t>(stream)));
 }
 
 size_t b200awq_w4a16_gemm_workspace_bytes(int, int, int) { return 0; }
@@ -355,7 +357,8 @@ int b200awq_w4a16_gemm(const void* x, const void* qweight, const void* scales, c
   (void)workspace_bytes;
   if (int e = check_common(x, qweight, scales, szeros, y, m, n, k, group_size, dtype)) return e;
   if (n % 128) return B200AWQ_ERR_SHAPE;  // reference: N / CTA_N with CTA_N = 128, gemm_cuda.cu:38,1225
-  return counted(launch_gemm(x, qweight, scales, szeros, y, m, n, k, dtype, static_cast<cudaStream_t>(stream)), true);
+  const W4Operands o{x, qweight, scales, szeros, y, m, n, k, dtype, static_cast<cudaStream_t>(stream)};
+  return counted(launch_w4a16(o, Envelope::kGemm));
 }
 
 // ---------------------------------------------------------------- W8A8
@@ -366,8 +369,7 @@ int b200awq_w8a8_gemm(const void* x, const void* w, const void* wscales, const v
   if ((reinterpret_cast<uintptr_t>(wscales) | reinterpret_cast<uintptr_t>(ascales) | reinterpret_cast<uintptr_t>(bias)) & 1u)
     return B200AWQ_ERR_ALIGN;
   if (int e = check_device()) return e;
-  return counted(b200awq::launch_w8a8_gemm(x, w, wscales, ascales, bias, y, m, n, k, pdl_enabled(), static_cast<cudaStream_t>(stream)),
-                 true);
+  return counted(b200awq::launch_w8a8_gemm(x, w, wscales, ascales, bias, y, m, n, k, pdl_enabled(), static_cast<cudaStream_t>(stream)));
 }
 
 namespace {

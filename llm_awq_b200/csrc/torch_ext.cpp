@@ -26,8 +26,16 @@ int dtype_code(const torch::Tensor& t, const char* fn) {
   TORCH_CHECK(false, fn, " failed to dispatch data type ", t.scalar_type());
 }
 
-void check_inputs(const torch::Tensor& in, const torch::Tensor& kernel, const torch::Tensor& scales,
-                  const torch::Tensor& zeros) {
+// Operands of one W4A16 product: in_feats [..., k] (m rows), qweight int16 [n / 4, k], scales / zeros [>= k / group, n]
+// of in_feats' dtype, all CUDA and contiguous.  The output has in_feats' shape with n channels.
+struct W4Shape {
+  int64_t m, n, k;
+  int dt;
+  std::vector<int64_t> out_shape;
+};
+
+W4Shape w4a16_shape(const torch::Tensor& in, const torch::Tensor& kernel, const torch::Tensor& scales,
+                    const torch::Tensor& zeros, int64_t group_size, const char* fn) {
   TORCH_CHECK(in.is_cuda() && kernel.is_cuda() && scales.is_cuda() && zeros.is_cuda(), "all tensors must be CUDA tensors");
   TORCH_CHECK(scales.scalar_type() == in.scalar_type());  // reference: gemv_cuda.cu:260, gemm_cuda.cu:1145
   TORCH_CHECK(zeros.scalar_type() == in.scalar_type());   // reference: gemv_cuda.cu:261, gemm_cuda.cu:1146
@@ -35,9 +43,18 @@ void check_inputs(const torch::Tensor& in, const torch::Tensor& kernel, const to
   TORCH_CHECK(in.is_contiguous() && kernel.is_contiguous() && scales.is_contiguous() && zeros.is_contiguous(),
               "inputs must be contiguous");
   TORCH_CHECK(kernel.dim() == 2 && scales.dim() == 2 && zeros.dim() == 2 && in.dim() >= 1, "bad tensor ranks");
+  const int dt = dtype_code(in, fn);
+  const int64_t n = kernel.size(0) * 4, k = in.size(-1);  // n: reference gemm_cuda.cu:1133
+  TORCH_CHECK(k > 0, fn, ": in_feats must have a non-empty last dimension");
+  TORCH_CHECK(kernel.size(1) == k, "qweight does not match in_feats");
+  TORCH_CHECK(scales.size(1) == n && zeros.size(1) == n && scales.size(0) * group_size >= k && zeros.size(0) * group_size >= k,
+              "scales / zeros do not match (n, k, group)");
+  std::vector<int64_t> out_shape = in.sizes().vec();
+  out_shape.back() = n;
+  return {in.numel() / k, n, k, dt, out_shape};
 }
 
-void raise(int code, bool is_gemv) {
+void raise(int code, bool is_gemv = false) {
   if (code == 0) return;
   // the reference throws std::runtime_error for unsupported batch / group (gemv_cuda.cu:329,334)
   if (is_gemv && code == B200AWQ_ERR_BATCH) throw std::runtime_error("Unsupported batch size for gemv kernel.\n");
@@ -45,49 +62,34 @@ void raise(int code, bool is_gemv) {
   TORCH_CHECK(false, "b200awq: ", b200awq_strerror(code), " (code ", code, ")");
 }
 
+void* current_stream() { return at::cuda::getCurrentCUDAStream().stream(); }
+
 }  // namespace
 
 torch::Tensor gemv_forward_cuda_new(torch::Tensor _in_feats, torch::Tensor _kernel, torch::Tensor _scaling_factors,
                                     torch::Tensor _zeros, int m, int n, int k, int group_size) {
-  check_inputs(_in_feats, _kernel, _scaling_factors, _zeros);
-  const int dt = dtype_code(_in_feats, "gemv_forward_cuda_new");
-  TORCH_CHECK(_in_feats.size(-1) == k && _in_feats.numel() == (int64_t)m * k, "in_feats does not match (m, k)");
-  TORCH_CHECK(_kernel.size(0) * 4 == n && _kernel.size(1) == k, "qweight does not match (n, k)");
-  TORCH_CHECK(_scaling_factors.size(1) == n && _zeros.size(1) == n && _scaling_factors.size(0) * group_size >= k &&
-                  _zeros.size(0) * group_size >= k,
-              "scales / zeros do not match (n, k, group)");
+  const W4Shape s = w4a16_shape(_in_feats, _kernel, _scaling_factors, _zeros, group_size, "gemv_forward_cuda_new");
+  TORCH_CHECK(s.k == k && s.m == m, "in_feats does not match (m, k)");
+  TORCH_CHECK(s.n == n, "qweight does not match (n, k)");
   const c10::cuda::CUDAGuard guard(_in_feats.device());
-  std::vector<int64_t> output_shape = _in_feats.sizes().vec();
-  output_shape.back() = n;
-  at::Tensor out = torch::empty(output_shape, _in_feats.options());
+  at::Tensor out = torch::empty(s.out_shape, _in_feats.options());
   raise(b200awq_w4a16_gemv(_in_feats.data_ptr(), _kernel.data_ptr(), _scaling_factors.data_ptr(), _zeros.data_ptr(),
-                           out.data_ptr(), m, n, k, group_size, dt, at::cuda::getCurrentCUDAStream().stream()),
+                           out.data_ptr(), m, n, k, group_size, s.dt, current_stream()),
         true);
   return out;
 }
 
 torch::Tensor gemm_forward_cuda_new(torch::Tensor _in_feats, torch::Tensor _kernel, torch::Tensor _scales,
                                     torch::Tensor _zeros) {
-  check_inputs(_in_feats, _kernel, _scales, _zeros);
-  const int dt = dtype_code(_in_feats, "gemm_forward_cuda_new");
-  const int64_t k = _in_feats.size(-1);
-  const int64_t n = _kernel.size(0) * 4;  // reference: gemm_cuda.cu:1133
-  const int64_t m = _in_feats.numel() / k;
-  TORCH_CHECK(_kernel.size(1) == k, "qweight does not match in_feats");
-  TORCH_CHECK(_scales.size(1) == n && _zeros.size(1) == n && _scales.size(0) * 128 >= k && _zeros.size(0) * 128 >= k,
-              "scales / zeros do not match (n, k)");
+  const W4Shape s = w4a16_shape(_in_feats, _kernel, _scales, _zeros, 128, "gemm_forward_cuda_new");
   const c10::cuda::CUDAGuard guard(_in_feats.device());
-  std::vector<int64_t> output_shape = _in_feats.sizes().vec();
-  output_shape.back() = n;
-  at::Tensor out = torch::empty(output_shape, _in_feats.options());
-  if (m == 0) return out;
-  const size_t ws_bytes = b200awq_w4a16_gemm_workspace_bytes((int)m, (int)n, (int)k);
+  at::Tensor out = torch::empty(s.out_shape, _in_feats.options());
+  if (s.m == 0) return out;
+  const size_t ws_bytes = b200awq_w4a16_gemm_workspace_bytes((int)s.m, (int)s.n, (int)s.k);
   at::Tensor ws;
   if (ws_bytes) ws = torch::empty({(int64_t)ws_bytes}, _in_feats.options().dtype(torch::kUInt8));
   raise(b200awq_w4a16_gemm(_in_feats.data_ptr(), _kernel.data_ptr(), _scales.data_ptr(), _zeros.data_ptr(), out.data_ptr(),
-                           (int)m, (int)n, (int)k, 128, dt, ws_bytes ? ws.data_ptr() : nullptr, ws_bytes,
-                           at::cuda::getCurrentCUDAStream().stream()),
-        false);
+                           (int)s.m, (int)s.n, (int)s.k, 128, s.dt, ws_bytes ? ws.data_ptr() : nullptr, ws_bytes, current_stream()));
   return out;
 }
 
@@ -99,17 +101,7 @@ torch::Tensor w4a16_linear_forward_cuda(torch::Tensor _in_feats, torch::Tensor _
                                         torch::Tensor _zeros, int64_t group_size, c10::optional<torch::Tensor> bias,
                                         c10::optional<torch::Tensor> residual) {
   const char* fn = "w4a16_linear_forward_cuda";
-  check_inputs(_in_feats, _kernel, _scales, _zeros);
-  const int dt = dtype_code(_in_feats, fn);
-  const int64_t k = _in_feats.size(-1);
-  const int64_t n = _kernel.size(0) * 4;
-  const int64_t m = k ? _in_feats.numel() / k : 0;
-  TORCH_CHECK(_kernel.size(1) == k, "qweight does not match in_feats");
-  TORCH_CHECK(_scales.size(1) == n && _zeros.size(1) == n && _scales.size(0) * group_size >= k &&
-                  _zeros.size(0) * group_size >= k,
-              "scales / zeros do not match (n, k, group)");
-  std::vector<int64_t> output_shape = _in_feats.sizes().vec();
-  output_shape.back() = n;
+  const W4Shape s = w4a16_shape(_in_feats, _kernel, _scales, _zeros, group_size, fn);
   for (const c10::optional<torch::Tensor>* t : {&bias, &residual}) {
     if (!t->has_value()) continue;
     const torch::Tensor& v = t->value();
@@ -117,18 +109,17 @@ torch::Tensor w4a16_linear_forward_cuda(torch::Tensor _in_feats, torch::Tensor _
     TORCH_CHECK(v.scalar_type() == _in_feats.scalar_type(), fn, ": bias / residual must have in_feats' dtype");
     TORCH_CHECK(v.is_contiguous(), fn, ": bias / residual must be contiguous");
   }
-  if (bias.has_value()) TORCH_CHECK(bias->dim() == 1 && bias->size(0) == n, fn, ": bias must be [", n, "]");
+  if (bias.has_value()) TORCH_CHECK(bias->dim() == 1 && bias->size(0) == s.n, fn, ": bias must be [", s.n, "]");
   if (residual.has_value())
-    TORCH_CHECK(residual->sizes() == torch::IntArrayRef(output_shape), fn, ": residual must have the output's shape ",
-                torch::IntArrayRef(output_shape));
+    TORCH_CHECK(residual->sizes() == torch::IntArrayRef(s.out_shape), fn, ": residual must have the output's shape ",
+                torch::IntArrayRef(s.out_shape));
   const c10::cuda::CUDAGuard guard(_in_feats.device());
-  at::Tensor out = torch::empty(output_shape, _in_feats.options());
-  if (m == 0) return out;
+  at::Tensor out = torch::empty(s.out_shape, _in_feats.options());
+  if (s.m == 0) return out;
   raise(b200awq_w4a16_linear(_in_feats.data_ptr(), _kernel.data_ptr(), _scales.data_ptr(), _zeros.data_ptr(),
                              bias.has_value() ? bias->data_ptr() : nullptr,
-                             residual.has_value() ? residual->data_ptr() : nullptr, out.data_ptr(), (int)m, (int)n, (int)k,
-                             (int)group_size, dt, at::cuda::getCurrentCUDAStream().stream()),
-        false);
+                             residual.has_value() ? residual->data_ptr() : nullptr, out.data_ptr(), (int)s.m, (int)s.n,
+                             (int)s.k, (int)group_size, s.dt, current_stream()));
   return out;
 }
 
@@ -137,38 +128,26 @@ torch::Tensor w4a16_linear_forward_cuda(torch::Tensor _in_feats, torch::Tensor _
 torch::Tensor mlp_front_forward_cuda(torch::Tensor _in_feats, torch::Tensor _gate_kernel, torch::Tensor _gate_scales,
                                      torch::Tensor _gate_zeros, torch::Tensor _up_kernel, torch::Tensor _up_scales,
                                      torch::Tensor _up_zeros) {
-  check_inputs(_in_feats, _gate_kernel, _gate_scales, _gate_zeros);
-  check_inputs(_in_feats, _up_kernel, _up_scales, _up_zeros);
-  const int dt = dtype_code(_in_feats, "mlp_front_forward_cuda");
-  const int64_t k = _in_feats.size(-1);
-  const int64_t n = _gate_kernel.size(0) * 4;
-  const int64_t m = _in_feats.numel() / k;
-  TORCH_CHECK(_gate_kernel.size(1) == k && _up_kernel.size(0) * 4 == n && _up_kernel.size(1) == k, "qweights do not match");
-  for (const torch::Tensor* t : {&_gate_scales, &_gate_zeros, &_up_scales, &_up_zeros})
-    TORCH_CHECK(t->size(1) == n && t->size(0) * 128 >= k, "scales / zeros do not match (n, k)");
+  const char* fn = "mlp_front_forward_cuda";
+  const W4Shape s = w4a16_shape(_in_feats, _gate_kernel, _gate_scales, _gate_zeros, 128, fn);
+  TORCH_CHECK(w4a16_shape(_in_feats, _up_kernel, _up_scales, _up_zeros, 128, fn).n == s.n, "qweights do not match");
   const c10::cuda::CUDAGuard guard(_in_feats.device());
-  std::vector<int64_t> output_shape = _in_feats.sizes().vec();
-  output_shape.back() = n;
-  at::Tensor out = torch::empty(output_shape, _in_feats.options());
-  if (m == 0) return out;
-  at::Tensor ws;
-  size_t ws_bytes = 0;
-  if (!(m == 1 && dt == B200AWQ_DTYPE_F16)) {
-    ws_bytes = b200awq_w4a16_mlp_front_workspace_bytes((int)m, (int)n, (int)k);
-    ws = torch::empty({(int64_t)ws_bytes}, _in_feats.options().dtype(torch::kUInt8));
-  }
-  int rc = b200awq_w4a16_mlp_front(_in_feats.data_ptr(), _gate_kernel.data_ptr(), _gate_scales.data_ptr(), _gate_zeros.data_ptr(),
-                                   _up_kernel.data_ptr(), _up_scales.data_ptr(), _up_zeros.data_ptr(), out.data_ptr(), (int)m,
-                                   (int)n, (int)k, 128, dt, ws_bytes ? ws.data_ptr() : nullptr, ws_bytes,
-                                   at::cuda::getCurrentCUDAStream().stream());
-  if (rc == B200AWQ_ERR_WORKSPACE && ws_bytes == 0) {  // the one-kernel path declined the shape: composed path
-    ws_bytes = b200awq_w4a16_mlp_front_workspace_bytes((int)m, (int)n, (int)k);
-    ws = torch::empty({(int64_t)ws_bytes}, _in_feats.options().dtype(torch::kUInt8));
-    rc = b200awq_w4a16_mlp_front(_in_feats.data_ptr(), _gate_kernel.data_ptr(), _gate_scales.data_ptr(), _gate_zeros.data_ptr(),
-                                 _up_kernel.data_ptr(), _up_scales.data_ptr(), _up_zeros.data_ptr(), out.data_ptr(), (int)m, (int)n,
-                                 (int)k, 128, dt, ws.data_ptr(), ws_bytes, at::cuda::getCurrentCUDAStream().stream());
-  }
-  raise(rc, false);
+  at::Tensor out = torch::empty(s.out_shape, _in_feats.options());
+  if (s.m == 0) return out;
+  // One fp16 token first tries the fused kernel, which needs no workspace; B200AWQ_ERR_WORKSPACE means that it declined
+  // the shape and the composed path needs one.
+  auto call = [&](bool with_workspace) {
+    const size_t bytes = with_workspace ? b200awq_w4a16_mlp_front_workspace_bytes((int)s.m, (int)s.n, (int)s.k) : 0;
+    const at::Tensor ws = bytes ? torch::empty({(int64_t)bytes}, _in_feats.options().dtype(torch::kUInt8)) : at::Tensor();
+    return b200awq_w4a16_mlp_front(_in_feats.data_ptr(), _gate_kernel.data_ptr(), _gate_scales.data_ptr(),
+                                   _gate_zeros.data_ptr(), _up_kernel.data_ptr(), _up_scales.data_ptr(), _up_zeros.data_ptr(),
+                                   out.data_ptr(), (int)s.m, (int)s.n, (int)s.k, 128, s.dt, bytes ? ws.data_ptr() : nullptr,
+                                   bytes, current_stream());
+  };
+  const bool fused_first = s.m == 1 && s.dt == B200AWQ_DTYPE_F16;
+  int rc = call(!fused_first);
+  if (fused_first && rc == B200AWQ_ERR_WORKSPACE) rc = call(true);
+  raise(rc);
   return out;
 }
 
@@ -187,8 +166,7 @@ void layernorm_forward_cuda(torch::Tensor _input, torch::Tensor _gamma, torch::T
   if (_input.numel() == 0) return;
   const c10::cuda::CUDAGuard guard(_input.device());
   raise(b200awq_rmsnorm(_input.data_ptr(), _gamma.data_ptr(), _out.data_ptr(), (int)(_input.numel() / n), (int)n, eps, dt,
-                        at::cuda::getCurrentCUDAStream().stream()),
-        false);
+                        current_stream()));
 }
 
 namespace {
@@ -206,7 +184,7 @@ const torch::Tensor& attention_workspace(const torch::Tensor& like, size_t need)
     std::vector<torch::Tensor> replaced;  // still referenced by graphs captured before a growth
   };
   static auto& workspaces = *new std::map<std::pair<int, void*>, Buffers>();
-  Buffers& w = workspaces[std::make_pair((int)like.get_device(), (void*)at::cuda::getCurrentCUDAStream().stream())];
+  Buffers& w = workspaces[std::make_pair((int)like.get_device(), current_stream())];
   const size_t have = w.current.defined() ? (size_t)w.current.numel() : 0;
   if (have < need) {
     if (w.current.defined()) w.replaced.push_back(w.current);
@@ -254,9 +232,7 @@ torch::Tensor single_query_attention(const torch::Tensor q, const torch::Tensor 
   raise(b200awq_single_query_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
                                        out.data_ptr(), lps, batch_size, nheads, nheads_kv, headdim, memory_max_seqlen, timestep,
                                        (long long)q.stride(0), (long long)k.stride(0), (long long)v.stride(0), rotary_embedding_dim, rotary_base, rotary_scale,
-                                       neox_rotary_style ? 1 : 0, dt, ws.data_ptr(), (size_t)ws.numel(),
-                                       at::cuda::getCurrentCUDAStream().stream()),
-        false);
+                                       neox_rotary_style ? 1 : 0, dt, ws.data_ptr(), (size_t)ws.numel(), current_stream()));
   return out;
 }
 
@@ -273,8 +249,7 @@ at::Tensor fused_rope_with_pos_forward_func(const at::Tensor& input, const at::T
   const long long os[4] = {output.stride(0), output.stride(1), output.stride(2), output.stride(3)};
   const c10::cuda::CUDAGuard guard(input.device());
   raise(b200awq_rope_with_pos(input.data_ptr(), freqs.data_ptr<float>(), output.data_ptr(), s, b, h, d, d2, is, os, dt,
-                              at::cuda::getCurrentCUDAStream().stream()),
-        false);
+                              current_stream()));
   return output;
 }
 
@@ -297,9 +272,7 @@ void rotary_embedding_neox(at::Tensor& positions, at::Tensor& query, at::Tensor&
   const c10::cuda::CUDAGuard guard(query.device());
   raise(b200awq_rotary_embedding_neox(reinterpret_cast<const long long*>(positions.data_ptr<int64_t>()), query.data_ptr(),
                                       key.data_ptr(), cos_sin_cache.data_ptr(), (int)tokens, (int)q_heads, (int)k_heads,
-                                      head_size, (int)rot_dim, q_heads * head_size, k_heads * head_size, dt,
-                                      at::cuda::getCurrentCUDAStream().stream()),
-        false);
+                                      head_size, (int)rot_dim, q_heads * head_size, k_heads * head_size, dt, current_stream()));
 }
 
 // ---------------------------------------------------------------- W8A8 (w8a8/*.cu of the reference)
@@ -340,8 +313,7 @@ void w8a8_gemm(const torch::Tensor& in, const torch::Tensor& kernel, const torch
   if (m == 0 || n == 0) return;
   const c10::cuda::CUDAGuard guard(in.device());
   raise(b200awq_w8a8_gemm(in.data_ptr(), kernel.data_ptr(), wscales.data_ptr(), ascales.data_ptr(), bias ? bias->data_ptr() : nullptr,
-                          out.data_ptr(), (int)m, (int)n, (int)k, at::cuda::getCurrentCUDAStream().stream()),
-        false);
+                          out.data_ptr(), (int)m, (int)n, (int)k, current_stream()));
 }
 
 int act_dtype(const torch::Tensor& t, const char* fn) {
@@ -374,9 +346,7 @@ void invoke_quant(torch::Tensor& out, torch::Tensor& input, torch::Tensor& scale
   const int64_t n = input.size(-1), m = input.numel() / n;
   TORCH_CHECK(out.numel() == input.numel() && scale.numel() >= m, fn, ": out must match input, scale needs one per token");
   const c10::cuda::CUDAGuard guard(input.device());
-  raise(b200awq_quant_per_token(input.data_ptr(), out.data_ptr(), scale.data_ptr(), (int)m, (int)n, dt,
-                                at::cuda::getCurrentCUDAStream().stream()),
-        false);
+  raise(b200awq_quant_per_token(input.data_ptr(), out.data_ptr(), scale.data_ptr(), (int)m, (int)n, dt, current_stream()));
 }
 
 // reference: w8a8/layernorm.cu:193-231
@@ -403,8 +373,7 @@ void rms_norm_general(torch::Tensor& out, torch::Tensor& input, torch::Tensor& w
   }
   const c10::cuda::CUDAGuard guard(input.device());
   raise(b200awq_layernorm_quant(input.data_ptr(), weight.data_ptr(), beta, out.data_ptr(), scaling.data_ptr(), (int)m, (int)n,
-                                epsilon, use_per_token_quant ? 1 : 0, dt, at::cuda::getCurrentCUDAStream().stream()),
-        false);
+                                epsilon, use_per_token_quant ? 1 : 0, dt, current_stream()));
 }
 
 // reference: w8a8/act.cu:120-141 (input [..., 2d] -> new tensor [..., d])
@@ -419,8 +388,7 @@ torch::Tensor silu_and_mul(torch::Tensor& input) {
   torch::Tensor out = torch::empty(shape, input.options());
   if (m == 0 || d == 0) return out;
   const c10::cuda::CUDAGuard guard(input.device());
-  raise(b200awq_silu_and_mul(input.data_ptr(), out.data_ptr(), (int)m, (int)d, dt, at::cuda::getCurrentCUDAStream().stream()),
-        false);
+  raise(b200awq_silu_and_mul(input.data_ptr(), out.data_ptr(), (int)m, (int)d, dt, current_stream()));
   return out;
 }
 
@@ -438,8 +406,7 @@ void gelu_and_quant(torch::Tensor& out, torch::Tensor& input, torch::Tensor& sca
               ": out / tmp must match input, scale_out needs one per token");
   const c10::cuda::CUDAGuard guard(input.device());
   raise(b200awq_gelu_quant(input.data_ptr(), out.data_ptr(), scale_out.data_ptr(), tmp.data_ptr(), (int)m, (int)n,
-                           at::cuda::getCurrentCUDAStream().stream()),
-        false);
+                           current_stream()));
 }
 
 // ---------------------------------------------------------------- attention over many queries
@@ -466,30 +433,51 @@ void check_attention_args(const torch::Tensor& q, const torch::Tensor& k, const 
               ": query and key / value must have the same dtype");
 }
 
+// What both attention wrappers hand the C entries for q, under the device guard: q as the TMA can read it, its strides,
+// the softmax scale (flash-attn's default 1 / sqrt(head_dim)) and the dtype code.
+struct AttentionQuery {
+  torch::Tensor q;
+  long long strides[3];
+  float scale;
+  int dt;
+};
+
+AttentionQuery attention_query(const torch::Tensor& q_in, c10::optional<double> softmax_scale, const char* fn) {
+  torch::Tensor q = tma_ready(q_in);
+  const float scale = softmax_scale.has_value() ? (float)softmax_scale.value() : 1.0f / std::sqrt((float)q.size(-1));
+  return {q, {q.stride(0), q.stride(1), q.stride(2)}, scale, dtype_code(q, fn)};
+}
+
+// attention_workspace() when a call needs one: (nullptr, 0) for need == 0
+std::pair<void*, size_t> attention_workspace_if(const torch::Tensor& like, size_t need) {
+  if (!need) return {nullptr, 0};
+  const torch::Tensor& ws = attention_workspace(like, need);
+  return {ws.data_ptr(), (size_t)ws.numel()};
+}
+
 torch::Tensor run_prefill_attention(const torch::Tensor& q_in, const torch::Tensor& k_in, const torch::Tensor& v_in,
                                     torch::Tensor& out, const int* cu_seqlens, int batch, int seqlen_q, int seqlen_k,
-                                    c10::optional<double> softmax_scale, bool causal) {
+                                    c10::optional<double> softmax_scale, bool causal, const char* fn) {
   const c10::cuda::CUDAGuard guard(q_in.device());
-  const torch::Tensor q = tma_ready(q_in), k = tma_ready(k_in), v = tma_ready(v_in);
+  const AttentionQuery a = attention_query(q_in, softmax_scale, fn);
+  const torch::Tensor& q = a.q;
+  const torch::Tensor k = tma_ready(k_in), v = tma_ready(v_in);
   const int heads = q.size(-2), kv_heads = k.size(-2), d = q.size(-1);
-  const float scale = softmax_scale.has_value() ? (float)softmax_scale.value() : 1.0f / std::sqrt((float)d);
-  const long long qs[3] = {q.stride(0), q.stride(1), q.stride(2)};
   const long long ks[3] = {k.stride(0), k.stride(1), k.stride(2)};
   const long long vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
-  const int dt = q.scalar_type() == at::ScalarType::Half ? B200AWQ_DTYPE_F16 : B200AWQ_DTYPE_BF16;
-  void* st = at::cuda::getCurrentCUDAStream().stream();
   int rc = B200AWQ_ERR_SHAPE;
   if (!cu_seqlens) {  // few queries per KV head: the split-key kernel; outside its envelope the prefill kernel
-    const size_t need = b200awq_splitkv_attention_workspace_bytes(batch, seqlen_q, seqlen_k, heads, kv_heads, d);
-    const torch::Tensor* ws = need ? &attention_workspace(q, need) : nullptr;
+    const auto ws = attention_workspace_if(
+        q, b200awq_splitkv_attention_workspace_bytes(batch, seqlen_q, seqlen_k, heads, kv_heads, d));
     rc = b200awq_splitkv_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), batch, seqlen_q, seqlen_k, heads,
-                                   kv_heads, d, qs, ks, vs, scale, causal ? 1 : 0, dt, ws ? ws->data_ptr() : nullptr,
-                                   ws ? (size_t)ws->numel() : 0, st);
+                                   kv_heads, d, a.strides, ks, vs, a.scale, causal ? 1 : 0, a.dt, ws.first, ws.second,
+                                   current_stream());
   }
   if (rc == B200AWQ_ERR_SHAPE)
     rc = b200awq_prefill_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), cu_seqlens, cu_seqlens, batch,
-                                   seqlen_q, seqlen_k, heads, kv_heads, d, qs, ks, vs, scale, causal ? 1 : 0, dt, st);
-  raise(rc, false);
+                                   seqlen_q, seqlen_k, heads, kv_heads, d, a.strides, ks, vs, a.scale, causal ? 1 : 0, a.dt,
+                                   current_stream());
+  raise(rc);
   return out;
 }
 
@@ -504,7 +492,7 @@ torch::Tensor flash_attn_func(const torch::Tensor& q, const torch::Tensor& k, co
   TORCH_CHECK(k.sizes() == v.sizes(), fn, ": k and v must have the same shape");
   TORCH_CHECK(k.size(0) == q.size(0) && k.size(3) == q.size(3), fn, ": k / v batch and head_dim must match q");
   torch::Tensor out = torch::empty(q.sizes(), q.options());
-  return run_prefill_attention(q, k, v, out, nullptr, q.size(0), q.size(1), k.size(1), softmax_scale, causal);
+  return run_prefill_attention(q, k, v, out, nullptr, q.size(0), q.size(1), k.size(1), softmax_scale, causal, fn);
 }
 
 // qkv [total, 3, H, D], cu_seqlens int32 [batch + 1] -> out [total, H, D]
@@ -522,7 +510,7 @@ torch::Tensor flash_attn_varlen_qkvpacked_func(const torch::Tensor& qkv, const t
   torch::Tensor out = torch::empty({qkv.size(0), qkv.size(2), qkv.size(3)}, qkv.options());
   // [total, H, D] views as [1, total, H, D]: the batch stride is ignored for packed sequences
   return run_prefill_attention(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), out, cu_seqlens.data_ptr<int>(),
-                               (int)cu_seqlens.numel() - 1, (int)max_seqlen, (int)max_seqlen, softmax_scale, causal);
+                               (int)cu_seqlens.numel() - 1, (int)max_seqlen, (int)max_seqlen, softmax_scale, causal, fn);
 }
 
 // Attention of a chunk q [B, Sq, H, D] over keys [0, seqlen_k) of a KV cache, read in place -> out [B, Sq, H, D].  The
@@ -555,20 +543,14 @@ torch::Tensor kv_cache_attention(const torch::Tensor& q_in, const torch::Tensor&
   TORCH_CHECK(seqlen_k >= 0 && seqlen_k <= max_len, fn, ": seqlen_k must be in [0, ", max_len, "]");
   TORCH_CHECK(max_len <= INT32_MAX && q_in.size(1) <= INT32_MAX, fn, ": sizes out of range");
   const c10::cuda::CUDAGuard guard(q_in.device());
-  const torch::Tensor q = tma_ready(q_in);
-  const int batch = (int)q.size(0), seqlen_q = (int)q.size(1), heads = (int)q.size(2);
-  torch::Tensor out = torch::empty({q.size(0), q.size(1), q.size(2), d}, q.options());
-  const float scale = softmax_scale.has_value() ? (float)softmax_scale.value() : 1.0f / std::sqrt((float)d);
-  const long long qs[3] = {q.stride(0), q.stride(1), q.stride(2)};
-  const int dt = q.scalar_type() == at::ScalarType::Half ? B200AWQ_DTYPE_F16 : B200AWQ_DTYPE_BF16;
-  const size_t need =
-      b200awq_kv_cache_attention_workspace_bytes(layout, batch, seqlen_q, (int)seqlen_k, heads, kv_heads, (int)d);
-  const torch::Tensor* ws = need ? &attention_workspace(q, need) : nullptr;
-  raise(b200awq_kv_cache_attention(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), out.data_ptr(), layout, batch, seqlen_q,
-                                   (int)seqlen_k, (int)max_len, heads, kv_heads, (int)d, qs, scale, causal ? 1 : 0, dt,
-                                   ws ? ws->data_ptr() : nullptr, ws ? (size_t)ws->numel() : 0,
-                                   at::cuda::getCurrentCUDAStream().stream()),
-        false);
+  const AttentionQuery a = attention_query(q_in, softmax_scale, fn);
+  const int batch = (int)a.q.size(0), seqlen_q = (int)a.q.size(1), heads = (int)a.q.size(2);
+  torch::Tensor out = torch::empty({a.q.size(0), a.q.size(1), a.q.size(2), d}, a.q.options());
+  const auto ws = attention_workspace_if(
+      a.q, b200awq_kv_cache_attention_workspace_bytes(layout, batch, seqlen_q, (int)seqlen_k, heads, kv_heads, (int)d));
+  raise(b200awq_kv_cache_attention(a.q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), out.data_ptr(), layout, batch,
+                                   seqlen_q, (int)seqlen_k, (int)max_len, heads, kv_heads, (int)d, a.strides, a.scale,
+                                   causal ? 1 : 0, a.dt, ws.first, ws.second, current_stream()));
   return out;
 }
 
