@@ -55,6 +55,22 @@ struct AttnCfg {
   static_assert(kQBytes % 1024 == 0 && kKBytes % 1024 == 0, "tiles must stay aligned to the swizzle repeat");
 };
 
+// The two consumer warpgroups take turns at the tensor core (named barriers 3 and 4): one issues its wgmmas (P V of
+// tile n and Q K^T of tile n + 1, one batch) while the other runs its softmax.  Warpgroup 1 lets warpgroup 0 go first
+// and skips its last hand-over, so that every barrier phase completes.  Both wait for the Q tile before the first.
+struct Turns {
+  int wg;
+  uint64_t* qfull;
+  __device__ __forceinline__ void first() const {
+    if (wg == 1) asm volatile("bar.arrive 3, 256;" ::: "memory");
+    mbar_wait(qfull, 0);
+  }
+  __device__ __forceinline__ void wait() const { asm volatile("bar.sync %0, 256;" ::"r"(3 + wg) : "memory"); }
+  __device__ __forceinline__ void pass(bool last) const {
+    if (!last || wg == 0) asm volatile("bar.arrive %0, 256;" ::"r"(4 - wg) : "memory");
+  }
+};
+
 // first row of the K / V tile n in the sequence: n * kBN, or, for packed sequences, shifted back to end at the
 // sequence's end (see the file comment)
 __device__ __forceinline__ int key_tile_start(int n, int sk, bool varlen) {
@@ -184,7 +200,7 @@ prefill_attention_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_
                         make_smem_desc(v_addr + C::kMain * kBN * 2 + kk * 16 * 32, 3, kBN * 32, 256), 1u);
     }
   };
-  // scale, mask and online softmax of tile n's S: P into pa, O rescaled
+  // mask and online softmax of tile n's S: P into pa, O rescaled
   auto softmax = [&](int n) {
     const int ks = key_tile_start(n, sk, varlen);
     const int k_lo = n * kBN;  // keys below k_lo belong to earlier tiles
@@ -198,95 +214,12 @@ prefill_attention_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_
         sc[i] = ok ? sc[i] : -INFINITY;
       }
     }
-    float mx_lo = m_lo, mx_hi = m_hi;  // running max of the raw scores
-#pragma unroll
-    for (int i = 0; i < 64; i += 4) {
-      mx_lo = fmaxf(mx_lo, fmaxf(sc[i], sc[i + 1]));
-      mx_hi = fmaxf(mx_hi, fmaxf(sc[i + 2], sc[i + 3]));
-    }
-#pragma unroll
-    for (int d = 1; d <= 2; d <<= 1) {
-      mx_lo = fmaxf(mx_lo, __shfl_xor_sync(0xffffffffu, mx_lo, d));
-      mx_hi = fmaxf(mx_hi, __shfl_xor_sync(0xffffffffu, mx_hi, d));
-    }
-    // p = exp2(scale_log2 * (s - max)) as one FFMA and one ex2.  A row that has seen no key yet keeps max -inf: its
-    // probabilities are exp2(-inf) = 0 and nothing is rescaled.
-    const float nb_lo = mx_lo == -INFINITY ? 0.f : -mx_lo * scale_log2;
-    const float nb_hi = mx_hi == -INFINITY ? 0.f : -mx_hi * scale_log2;
-    const float alpha_lo = ex2(fmaf(m_lo, scale_log2, nb_lo)), alpha_hi = ex2(fmaf(m_hi, scale_log2, nb_hi));
-    m_lo = mx_lo, m_hi = mx_hi;
-    float sum_lo = 0.f, sum_hi = 0.f;
-#pragma unroll
-    for (int i = 0; i < 64; i += 4) {
-      const float p0 = ex2(fmaf(sc[i], scale_log2, nb_lo)), p1 = ex2(fmaf(sc[i + 1], scale_log2, nb_lo));
-      const float p2 = ex2(fmaf(sc[i + 2], scale_log2, nb_hi)), p3 = ex2(fmaf(sc[i + 3], scale_log2, nb_hi));
-      sum_lo += p0 + p1, sum_hi += p2 + p3;
-      const int kk = i >> 3, half = (i >> 2) & 1;  // columns 8 (i / 4) + 2 t: k16 step i / 8, k + 8 when half
-      pa[kk][2 * half] = pack2<T>(p0, p1);
-      pa[kk][2 * half + 1] = pack2<T>(p2, p3);
-    }
-    l_lo = l_lo * alpha_lo + sum_lo, l_hi = l_hi * alpha_hi + sum_hi;
-#pragma unroll
-    for (int i = 0; i < DP / 2; i += 4) {
-      o[i] *= alpha_lo, o[i + 1] *= alpha_lo;
-      o[i + 2] *= alpha_hi, o[i + 3] *= alpha_hi;
-    }
+    online_softmax<T>(sc, pa, o, m_lo, m_hi, l_lo, l_hi, scale_log2);
   };
-  // The two warpgroups take turns at the tensor core (named barriers 3 and 4): one issues its wgmmas (P V of tile n
-  // and Q K^T of tile n + 1, one batch) while the other runs its softmax.  Warpgroup 1 lets warpgroup 0 go first and
-  // skips its last hand-over, so that every barrier phase completes.
-  auto turn_wait = [&]() { asm volatile("bar.sync %0, 256;" ::"r"(3 + wg) : "memory"); };
-  auto turn_pass = [&]() { asm volatile("bar.arrive %0, 256;" ::"r"(4 - wg) : "memory"); };
-
-  if (n_tiles > 0) {
-    if (wg == 1) asm volatile("bar.arrive 3, 256;" ::: "memory");
-    mbar_wait(qfull, 0);
-    mbar_wait(&full[0], 0);
-    turn_wait();
-    wgmma_fence();
-    issue_qk(0);
-    wgmma_commit();
-    turn_pass();
-    wgmma_wait<0>();
-    acc_fence(sc);
-    softmax(0);
-  }
-  int s = 0;
-  uint32_t ph = 0;
-  for (int n = 0; n + 1 < n_tiles; ++n) {
-    const int s1 = s + 1 == kStages ? 0 : s + 1;
-    const uint32_t ph1 = s1 == 0 ? ph ^ 1 : ph;
-    mbar_wait(&full[s1], ph1);
-    turn_wait();
-    wgmma_fence();
-    issue_pv(s);
-    issue_qk(s1);
-    wgmma_commit();
-    turn_pass();
-    wgmma_wait<0>();
-    acc_fence(o);
-    acc_fence(sc);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[s]);  // tile n's K and V have been read
-    softmax(n + 1);
-    s = s1, ph = ph1;
-  }
-  if (n_tiles > 0) {  // P V of the last tile
-    turn_wait();
-    wgmma_fence();
-    issue_pv(s);
-    wgmma_commit();
-    if (wg == 0) turn_pass();
-    wgmma_wait<0>();
-    acc_fence(o);
-  }
+  consume_tiles<kStages>(n_tiles, full, empty, lane, sc, o, Turns{wg, qfull}, issue_qk, issue_pv, softmax);
 
   // ------------------------------------------------ epilogue: O / l, rounded once, staged, 16-byte stores
-#pragma unroll
-  for (int d = 1; d <= 2; d <<= 1) {
-    l_lo += __shfl_xor_sync(0xffffffffu, l_lo, d);
-    l_hi += __shfl_xor_sync(0xffffffffu, l_hi, d);
-  }
+  row_sums(l_lo, l_hi);
   const float inv_lo = l_lo > 0.f ? 1.f / l_lo : 0.f, inv_hi = l_hi > 0.f ? 1.f / l_hi : 0.f;
 #pragma unroll
   for (int j = 0; j < DP / 8; ++j) {

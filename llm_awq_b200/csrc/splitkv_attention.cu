@@ -119,8 +119,7 @@ splitkv_attention_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_
   uint64_t* full = reinterpret_cast<uint64_t*>(kvs + kStages * C::kStageBytes);  // [kStages] TMA -> consumers
   uint64_t* empty = full + kStages;                // [kStages] consumer warps -> TMA
 
-  // this CTA's cell: KV head hk of batch row b, packed rows from r0 (kWG = 1: all R rows, grid (split, hk, b)).  Row
-  // counts are read where used, so that kWG = 1 compiles as the kernel did before kWG existed.
+  // this CTA's cell: KV head hk of batch row b, packed rows from r0 (kWG = 1: all R rows, grid (split, hk, b))
   const int split = blockIdx.x;
   const int hk = kWG == 1 ? (int)blockIdx.y : (int)(blockIdx.z % a.kv_heads);
   const int b = kWG == 1 ? (int)blockIdx.z : (int)(blockIdx.z / a.kv_heads);
@@ -221,7 +220,7 @@ splitkv_attention_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_
     for (int kk = 0; kk < kBN / 16; ++kk)
       wgmma_pv<T, D>(o, pa[kk], make_smem_desc(v_addr + kk * 16 * 128, 1, kBN * 128, 1024), 1u);
   };
-  // scale, mask and online softmax of tile n's S: P into pa, O rescaled
+  // mask and online softmax of tile n's S: P into pa, O rescaled
   auto softmax = [&](int n) {
     const int k0 = (t0 + n) * kBN;
     if (k0 + kBN > min(lim_lo, lim_hi)) {  // on the raw scores: scale_log2 > 0 keeps -inf the smallest value
@@ -231,81 +230,11 @@ splitkv_attention_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_
         sc[i] = key < ((i & 2) ? lim_hi : lim_lo) ? sc[i] : -INFINITY;
       }
     }
-    float mx_lo = m_lo, mx_hi = m_hi;
-#pragma unroll
-    for (int i = 0; i < 64; i += 4) {
-      mx_lo = fmaxf(mx_lo, fmaxf(sc[i], sc[i + 1]));
-      mx_hi = fmaxf(mx_hi, fmaxf(sc[i + 2], sc[i + 3]));
-    }
-#pragma unroll
-    for (int d = 1; d <= 2; d <<= 1) {
-      mx_lo = fmaxf(mx_lo, __shfl_xor_sync(0xffffffffu, mx_lo, d));
-      mx_hi = fmaxf(mx_hi, __shfl_xor_sync(0xffffffffu, mx_hi, d));
-    }
-    // a row that has seen no key yet keeps max -inf: its probabilities are exp2(-inf) = 0 and nothing is rescaled
-    const float nb_lo = mx_lo == -INFINITY ? 0.f : -mx_lo * scale_log2;
-    const float nb_hi = mx_hi == -INFINITY ? 0.f : -mx_hi * scale_log2;
-    const float alpha_lo = ex2(fmaf(m_lo, scale_log2, nb_lo)), alpha_hi = ex2(fmaf(m_hi, scale_log2, nb_hi));
-    m_lo = mx_lo, m_hi = mx_hi;
-    float sum_lo = 0.f, sum_hi = 0.f;
-#pragma unroll
-    for (int i = 0; i < 64; i += 4) {
-      const float p0 = ex2(fmaf(sc[i], scale_log2, nb_lo)), p1 = ex2(fmaf(sc[i + 1], scale_log2, nb_lo));
-      const float p2 = ex2(fmaf(sc[i + 2], scale_log2, nb_hi)), p3 = ex2(fmaf(sc[i + 3], scale_log2, nb_hi));
-      sum_lo += p0 + p1, sum_hi += p2 + p3;
-      const int kk = i >> 3, half = (i >> 2) & 1;  // columns 8 (i / 4) + 2 t: k16 step i / 8, k + 8 when half
-      pa[kk][2 * half] = pack2<T>(p0, p1);
-      pa[kk][2 * half + 1] = pack2<T>(p2, p3);
-    }
-    l_lo = l_lo * alpha_lo + sum_lo, l_hi = l_hi * alpha_hi + sum_hi;
-#pragma unroll
-    for (int i = 0; i < D / 2; i += 4) {
-      o[i] *= alpha_lo, o[i + 1] *= alpha_lo;
-      o[i + 2] *= alpha_hi, o[i + 3] *= alpha_hi;
-    }
+    online_softmax<T>(sc, pa, o, m_lo, m_hi, l_lo, l_hi, scale_log2);
   };
+  consume_tiles<kStages>(n_tiles, full, empty, lane, sc, o, NoTurns{}, issue_qk, issue_pv, softmax);
+  row_sums(l_lo, l_hi);
 
-  if (n_tiles > 0) {
-    mbar_wait(&full[0], 0);
-    wgmma_fence();
-    issue_qk(0);
-    wgmma_commit();
-    wgmma_wait<0>();
-    acc_fence(sc);
-    softmax(0);
-  }
-  int s = 0;
-  uint32_t ph = 0;
-  for (int n = 0; n + 1 < n_tiles; ++n) {
-    const int s1 = s + 1 == kStages ? 0 : s + 1;
-    const uint32_t ph1 = s1 == 0 ? ph ^ 1 : ph;
-    mbar_wait(&full[s1], ph1);
-    wgmma_fence();
-    issue_pv(s);
-    issue_qk(s1);
-    wgmma_commit();
-    wgmma_wait<0>();
-    acc_fence(o);
-    acc_fence(sc);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[s]);  // tile n's K and V have been read
-    softmax(n + 1);
-    s = s1, ph = ph1;
-  }
-  if (n_tiles > 0) {  // P V of the last tile
-    wgmma_fence();
-    issue_pv(s);
-    wgmma_commit();
-    wgmma_wait<0>();
-    acc_fence(o);
-  }
-#pragma unroll
-  for (int d = 1; d <= 2; d <<= 1) {
-    l_lo += __shfl_xor_sync(0xffffffffu, l_lo, d);
-    l_hi += __shfl_xor_sync(0xffffffffu, l_hi, d);
-  }
-
-  // declared here rather than with their peers above: kWG = 1 then compiles to the same code as before kWG existed
   const int lr_lo = r_lo - r0;        // this thread's rows in the cell: lr_lo, lr_lo + 8
   const int ctid = threadIdx.x;       // thread of the CTA's consumers
   const int n_threads = 128 * n_wg;   // consumer threads of this CTA
