@@ -1,6 +1,7 @@
 """Further parity cases: Llama-2-70B TP=1 / TP=8-shard shapes over the whole
 token sweep, the two known-answer tests SURVEY.md §8c(5) lists (all-ones weights, single non-zero group), the
-persistent ring kernel's partition edge cases, and its determinism."""
+persistent ring and decode kernels' partition edge cases (w4a16_plans.edge_cases for this device's SM count), and
+their determinism."""
 import ctypes
 
 import numpy as np
@@ -11,10 +12,18 @@ import llm_awq_b200 as P
 from oracle import w4a16_oracle as O
 from awq_testutil import abi_call, dt_name, gen_layer, gen_x, np64, oracle_forward, rel_err
 from test_gpu_parity import check
+from w4a16_plans import edge_cases
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 DTYPES = [torch.float16, torch.bfloat16]
+# the partition edges depend on the SM count; without a device the cases are only collected (and skipped)
+SMS = torch.cuda.get_device_properties(0).multi_processor_count if torch.cuda.is_available() else 132
+
+
+def edge_shapes(prefix):
+    """Distinct (n, k) of this device's edge cases whose label starts with `prefix`, in order."""
+    return list(dict.fromkeys((c.n, c.k) for c in edge_cases(SMS) if c.label.startswith(prefix)))
 
 
 def _call(x, qw, s, z, M, N, K, dtype):
@@ -83,12 +92,12 @@ def test_kat_single_nonzero_group(M, grp, dtype):
 # ------------------------------------------------------------------ ring kernel: partition edge cases
 @pytest.mark.parametrize("dtype", DTYPES, ids=["f16", "bf16"])
 @pytest.mark.parametrize("M", [1, 2, 4])
-@pytest.mark.parametrize("N,K", [(8, 2048), (16, 4096), (1184, 2048), (1192, 2176), (2376, 4224), (4744, 2048),
-                                 (296, 6144), (8, 128), (40, 1920)])
+@pytest.mark.parametrize("N,K", edge_shapes("ring"))
 def test_ring_partition_edges(N, K, M, dtype):
-    """Channel counts around multiples of an SM count (148 CTAs, 74 clusters: fewer octets than clusters, exactly
-    one / two per cluster, an odd octet at the end), odd group counts (k split 8|9, 16|17), k below the split
-    threshold, slots of fewer than 16 groups."""
+    """Octet counts around the number of ring units this device's SM count gives (fewer octets than units, exactly
+    one per unit, an odd octet at the end of a unit), unsplit (15 groups, one slot of fewer than 16 groups) and split
+    over two CTAs (17 groups: 8 | 9), and the k at which the activations leave too little room for the ring and the
+    next kernel takes the shape."""
     qw, s, z = gen_layer(N, K, dtype, seed=N + K, device=DEV)
     x = gen_x(M, K, dtype, seed=M + 1, device=DEV)
     y = _call(x, qw, s, z, M, N, K, dtype)
@@ -96,13 +105,12 @@ def test_ring_partition_edges(N, K, M, dtype):
 
 
 @pytest.mark.parametrize("slots", [0, 3])
-@pytest.mark.parametrize("N,K,split", [(N, K, s) for (N, K) in [(8, 512), (24, 1024), (592, 4096), (600, 4096), (2376, 4224),
-                                                                (4096, 4096), (1280, 8192), (4096, 14336), (4104, 11008),
-                                                                (8192, 1024)] for s in (1, 2, 4) if K // 128 >= s])
+@pytest.mark.parametrize("N,K,split", [(N, K, s) for (N, K) in edge_shapes("decode") for s in (1, 2, 4) if K // 128 >= s])
 def test_decode_kernel_splits_and_ring_depths(N, K, split, slots):
-    """The one-token decode kernel with the k split forced to 1 / 2 / 4 CTAs per cluster and with the shallowest ring:
-    quad-row counts below / around the CTA count, row blocks of 4 / 8 / 12 channels at the end of a CTA's range, pieces of
-    fewer than 32 groups (k = 11008: 86 groups), k splits that leave odd group counts."""
+    """The one-token decode kernel with the k split forced to 1 / 2 / 4 CTAs per cluster (through the test override
+    B200AWQ_DECODE_SPLIT) and with the shallowest ring (B200AWQ_DECODE_SLOTS), on the decode edge shapes of this
+    device's SM count: quad-row counts 2 below / at / 2 above 4 and 8 per CTA, which leave row blocks of 4 / 12 channels
+    at the end of some CTAs' ranges, pieces of fewer than 32 groups, k splits that leave odd group counts."""
     import os
     dtype = torch.float16
     os.environ["B200AWQ_DECODE_SPLIT"] = str(split)
