@@ -246,6 +246,27 @@ int b200awq_kv_cache_attention(const void* q, const void* k_cache, const void* v
 size_t b200awq_kv_cache_attention_workspace_bytes(int layout, int batch, int seqlen_q, int seqlen_k, int heads,
                                                   int kv_heads, int head_dim);
 
+/* RoPE of a chunk's q and k with the store of k and v into a KV cache, in one launch: for tinychat's chunked prefill
+ * and long_forward's decode, what the caller's two fused_rope_with_pos_forward_func calls (the second on k) and its
+ * k / v cache stores compute.
+ *   qkv      the fused qkv linear's output as [batch, seqlen, heads + 2 kv_heads, head_dim]: heads 0 .. heads - 1 are
+ *            q, the next kv_heads are k, the last kv_heads are v; strides in ELEMENTS for (batch, token, head), unit
+ *            element stride
+ *   freqs    fp32 [seqlen, head_dim]: angle f_i of token s is freqs[s * head_dim + i], the same for every batch row
+ *   k_cache, v_cache  in `layout` (B200AWQ_KV_FT or B200AWQ_KV_BTHD), as b200awq_kv_cache_attention reads them
+ * Every q and k head becomes y[i] = x[i] cos f_i + rot(x)[i] sin f_i in fp32, rounded once to T, with rot as in
+ * b200awq_rope_with_pos (d2 = head_dim): bit-identical to b200awq_rope_with_pos.  Rotated q is written back into the q
+ * heads of qkv; rotated k and the v heads are stored into cache slots [start_pos, start_pos + seqlen) of cache rows
+ * [0, batch).  The k and v heads of qkv, every other cache slot and every cache row >= batch are left as they were.
+ * heads % kv_heads == 0, head_dim % 8 == 0 and <= 256, max_len >= 1, start_pos >= 0 and start_pos + seqlen <= max_len
+ * (the ring of the decode cache does not wrap here), layout one of the two (else B200AWQ_ERR_SHAPE); qkv, freqs and
+ * the caches 16-byte aligned and qkv_strides multiples of 8 (else B200AWQ_ERR_ALIGN).  batch == 0 or seqlen == 0 is a
+ * no-op.  One launch, no workspace, no atomics; qkv and freqs are read after the launch's dependency wait, so either
+ * may be written by the launch right before it in the stream. */
+int b200awq_rope_kv_store(void* qkv, const float* freqs, void* k_cache, void* v_cache, int layout, int batch, int seqlen,
+                          int heads, int kv_heads, int head_dim, int max_len, int start_pos,
+                          const long long qkv_strides[3], int dtype, void* stream);
+
 /* ---- W8A8 (int8 weights, int8 per-token activations): the vision-tower ops of the reference's extension
  * (csrc/pybind.cpp:30-37), called by awq/quantize/w8a8_linear.py and tinychat's QuantSiglipEncoder /
  * QuantInternVisionEncoder.  Scales are fp16 everywhere (the reference reads them as at::Half).  fp32 activations,

@@ -18,6 +18,7 @@ EXT = os.path.join(HERE, "plugin", "awq_inference_engine" + sysconfig.get_config
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
 KERNEL_SRCS = ("api.cu", "w4a16_decode.cu", "w4a16_ring.cu", "w4a16_stream.cu", "w4a16_wgmma.cu", "rmsnorm.cu", "silu_mul.cu", "attention.cu", "rope_neox.cu",
+               "rope_kv_store.cu",
                "w8a8_wgmma.cu", "w8a8_rowops.cu", "prefill_attention.cu", "splitkv_attention.cu")
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
@@ -37,7 +38,7 @@ def _run(cmd):
 
 def build_lib(force=False):
     srcs = [os.path.join(CSRC, f) for f in KERNEL_SRCS]
-    deps = srcs + [os.path.join(CSRC, f) for f in ("w4_common.cuh", "w4a16_kernels.h", "rope_neox.cuh", "tma_wgmma.cuh", "w8a8_math.cuh",
+    deps = srcs + [os.path.join(CSRC, f) for f in ("w4_common.cuh", "w4a16_kernels.h", "rope_neox.cuh", "rope_kv_store.cuh", "tma_wgmma.cuh", "w8a8_math.cuh",
                                                  "attention_wgmma.cuh")] + \
         [os.path.join(INCLUDE, "b200awq.h"), __file__]
     if not force and _newer(LIB, deps):

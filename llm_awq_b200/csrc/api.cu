@@ -320,6 +320,23 @@ int b200awq_kv_cache_attention(const void* q, const void* k_cache, const void* v
                                                     workspace, workspace_bytes, static_cast<cudaStream_t>(stream)));
 }
 
+int b200awq_rope_kv_store(void* qkv, const float* freqs, void* k_cache, void* v_cache, int layout, int batch, int seqlen,
+                          int heads, int kv_heads, int head_dim, int max_len, int start_pos, const long long qkv_strides[3],
+                          int dtype, void* stream) {
+  if (int e = check_dtype(dtype)) return e;
+  if ((layout != B200AWQ_KV_FT && layout != B200AWQ_KV_BTHD) || batch < 0 || seqlen < 0 || heads < 1 || kv_heads < 1 ||
+      heads % kv_heads || head_dim < 8 || head_dim % 8 || head_dim > 256 || max_len < 1 || start_pos < 0 ||
+      (long long)start_pos + seqlen > max_len)
+    return B200AWQ_ERR_SHAPE;
+  if (!aligned16(qkv) || !aligned16(freqs) || !aligned16(k_cache) || !aligned16(v_cache)) return B200AWQ_ERR_ALIGN;
+  if (!qkv_strides || qkv_strides[0] % 8 || qkv_strides[1] % 8 || qkv_strides[2] % 8) return B200AWQ_ERR_ALIGN;
+  if (batch == 0 || seqlen == 0) return 0;
+  if (int e = check_device()) return e;
+  return counted(b200awq::launch_rope_kv_store(qkv, freqs, k_cache, v_cache, layout, batch, seqlen, heads, kv_heads, head_dim,
+                                               max_len, start_pos, qkv_strides, dtype, pdl_enabled(),
+                                               static_cast<cudaStream_t>(stream)));
+}
+
 int b200awq_rope_with_pos(const void* x, const float* freqs, void* y, int s, int b, int h, int d, int d2,
                           const long long in_strides[4], const long long out_strides[4], int dtype, void* stream) {
   if (int e = check_dtype(dtype)) return e;

@@ -21,6 +21,7 @@
 #include <algorithm>
 #include <cfloat>
 
+#include "rope_kv_store.cuh"
 #include "w4_common.cuh"
 #include "w4a16_kernels.h"
 
@@ -376,10 +377,9 @@ __global__ void __launch_bounds__(256) rope_with_pos_kernel(const RopeArgs a) {
     const T* sp = src + h_id * a.sh;
     float v = to_float<T>(sp[d_id * a.sd]);
     if (d_id < a.d2) {
-      float sn, cs;
-      sincosf(fr[d_id], &sn, &cs);
+      const RopeAngle ang = rope_angle(fr[d_id]);
       const float rot = (d_id + a.d2 / 2 < a.d2) ? -to_float<T>(sp[(d_id + a.d2 / 2) * a.sd]) : to_float<T>(sp[(d_id - a.d2 / 2) * a.sd]);
-      v = v * cs + rot * sn;  // fused_rope_with_pos.cu:52-57
+      v = rope_apply(v, rot, ang);  // fused_rope_with_pos.cu:52-57
     }
     dst[h_id * a.oh + d_id * a.od] = from_float<T>(v);
   }

@@ -481,6 +481,34 @@ torch::Tensor run_prefill_attention(const torch::Tensor& q_in, const torch::Tens
   return out;
 }
 
+// The KV caches of kv_cache_attention and rope_kv_store on `like`'s device, for head_dim d: the layout follows from
+// k_cache's rank (5-D: tinychat's decode cache k [Bc, Hkv, D / 8, Lmax, 8], v [Bc, Hkv, Lmax, D]; 4-D: long_forward's
+// [Bc, Lmax, Hkv, D] both), caches contiguous.
+struct KvCaches {
+  int layout, kv_heads;
+  int64_t rows, max_len;
+};
+
+KvCaches kv_caches(const torch::Tensor& like, const torch::Tensor& k_cache, const torch::Tensor& v_cache, int64_t d,
+                   const char* fn) {
+  TORCH_CHECK(k_cache.is_contiguous() && v_cache.is_contiguous(), fn, ": caches must be contiguous");
+  TORCH_CHECK(k_cache.device() == like.device() && v_cache.device() == like.device(), fn, ": tensors must be on one device");
+  KvCaches c;
+  if (k_cache.dim() == 5) {
+    c.layout = B200AWQ_KV_FT;
+    c.rows = k_cache.size(0), c.kv_heads = (int)k_cache.size(1), c.max_len = k_cache.size(3);
+    TORCH_CHECK(k_cache.size(2) * 8 == d && k_cache.size(4) == 8, fn, ": k_cache must be [batch, kv_heads, head_dim / 8, max_len, 8]");
+    TORCH_CHECK(v_cache.dim() == 4 && v_cache.sizes() == torch::IntArrayRef({c.rows, c.kv_heads, c.max_len, d}), fn,
+                ": v_cache must be [batch, kv_heads, max_len, head_dim]");
+  } else {
+    TORCH_CHECK(k_cache.dim() == 4, fn, ": k_cache must be 5-D (FasterTransformer layout) or 4-D [batch, max_len, kv_heads, head_dim]");
+    c.layout = B200AWQ_KV_BTHD;
+    c.rows = k_cache.size(0), c.max_len = k_cache.size(1), c.kv_heads = (int)k_cache.size(2);
+    TORCH_CHECK(k_cache.size(3) == d && v_cache.sizes() == k_cache.sizes(), fn, ": k_cache / v_cache must be [batch, max_len, kv_heads, head_dim]");
+  }
+  return c;
+}
+
 }  // namespace
 
 // q [B, Sq, H, D], k / v [B, Sk, Hkv, D] -> out [B, Sq, H, D]
@@ -522,23 +550,8 @@ torch::Tensor kv_cache_attention(const torch::Tensor& q_in, const torch::Tensor&
   const char* fn = "kv_cache_attention";
   check_attention_args(q_in, k_cache, v_cache, 0.0, fn);
   TORCH_CHECK(q_in.dim() == 4, fn, ": q must be [batch, seqlen_q, heads, head_dim]");
-  TORCH_CHECK(k_cache.is_contiguous() && v_cache.is_contiguous(), fn, ": caches must be contiguous");
-  TORCH_CHECK(k_cache.device() == q_in.device() && v_cache.device() == q_in.device(), fn, ": tensors must be on one device");
   const int64_t d = q_in.size(3);
-  int layout, kv_heads;
-  int64_t rows, max_len;
-  if (k_cache.dim() == 5) {
-    layout = B200AWQ_KV_FT;
-    rows = k_cache.size(0), kv_heads = (int)k_cache.size(1), max_len = k_cache.size(3);
-    TORCH_CHECK(k_cache.size(2) * 8 == d && k_cache.size(4) == 8, fn, ": k_cache must be [batch, kv_heads, head_dim / 8, max_len, 8]");
-    TORCH_CHECK(v_cache.dim() == 4 && v_cache.sizes() == torch::IntArrayRef({rows, kv_heads, max_len, d}), fn,
-                ": v_cache must be [batch, kv_heads, max_len, head_dim]");
-  } else {
-    TORCH_CHECK(k_cache.dim() == 4, fn, ": k_cache must be 5-D (FasterTransformer layout) or 4-D [batch, max_len, kv_heads, head_dim]");
-    layout = B200AWQ_KV_BTHD;
-    rows = k_cache.size(0), max_len = k_cache.size(1), kv_heads = (int)k_cache.size(2);
-    TORCH_CHECK(k_cache.size(3) == d && v_cache.sizes() == k_cache.sizes(), fn, ": k_cache / v_cache must be [batch, max_len, kv_heads, head_dim]");
-  }
+  const auto [layout, kv_heads, rows, max_len] = kv_caches(q_in, k_cache, v_cache, d, fn);
   TORCH_CHECK(q_in.size(0) <= rows, fn, ": q has ", q_in.size(0), " batch rows, the caches ", rows);
   TORCH_CHECK(seqlen_k >= 0 && seqlen_k <= max_len, fn, ": seqlen_k must be in [0, ", max_len, "]");
   TORCH_CHECK(max_len <= INT32_MAX && q_in.size(1) <= INT32_MAX, fn, ": sizes out of range");
@@ -552,6 +565,37 @@ torch::Tensor kv_cache_attention(const torch::Tensor& q_in, const torch::Tensor&
                                    seqlen_q, (int)seqlen_k, (int)max_len, heads, kv_heads, (int)d, a.strides, a.scale,
                                    causal ? 1 : 0, a.dt, ws.first, ws.second, current_stream()));
   return out;
+}
+
+// RoPE of a chunk's q and k with the store of k and v into the caches, one launch (include/b200awq.h,
+// b200awq_rope_kv_store).  qkv [B, S, H + 2 Hkv, D] is tinychat's xqkv view (last dimension contiguous); freqs fp32,
+// contiguous, S * D angles ([S, D] or tinychat's [S, 1, 1, D] slice), shared by all batch rows; caches as for
+// kv_cache_attention, Hkv read from them.  Returns the view qkv[:, :, :H], which holds the rotated q.
+torch::Tensor rope_kv_store(const torch::Tensor& qkv, const torch::Tensor& freqs, torch::Tensor& k_cache,
+                            torch::Tensor& v_cache, int64_t start_pos) {
+  const char* fn = "rope_kv_store";
+  TORCH_CHECK(qkv.is_cuda() && freqs.is_cuda() && k_cache.is_cuda() && v_cache.is_cuda(), fn, ": tensors must be CUDA tensors");
+  TORCH_CHECK(qkv.dim() == 4 && qkv.stride(3) == 1, fn, ": qkv must be [batch, seqlen, heads + 2 kv_heads, head_dim] with a contiguous last dimension");
+  const int dt = dtype_code(qkv, fn);
+  TORCH_CHECK(k_cache.scalar_type() == qkv.scalar_type() && v_cache.scalar_type() == qkv.scalar_type(), fn,
+              ": qkv and the caches must have the same dtype");
+  TORCH_CHECK(freqs.device() == qkv.device(), fn, ": tensors must be on one device");
+  TORCH_CHECK(freqs.scalar_type() == at::ScalarType::Float && freqs.is_contiguous(), fn, ": freqs must be contiguous float32");
+  const int64_t B = qkv.size(0), S = qkv.size(1), D = qkv.size(3);
+  TORCH_CHECK(freqs.numel() == S * D, fn, ": freqs must hold seqlen * head_dim = ", S * D, " angles, not ", freqs.numel());
+  const auto [layout, kv_heads, rows, max_len] = kv_caches(qkv, k_cache, v_cache, D, fn);
+  const int64_t H = qkv.size(2) - 2 * kv_heads;
+  TORCH_CHECK(H >= 1, fn, ": qkv has ", qkv.size(2), " heads, fewer than 2 * kv_heads + 1 = ", 2 * kv_heads + 1);
+  TORCH_CHECK(B <= rows, fn, ": qkv has ", B, " batch rows, the caches ", rows);
+  TORCH_CHECK(start_pos >= 0 && start_pos + S <= max_len, fn, ": slots [", start_pos, ", ", start_pos + S,
+              ") are not within the caches' ", max_len);
+  TORCH_CHECK(max_len <= INT32_MAX, fn, ": sizes out of range");
+  if (B == 0 || S == 0) return qkv.narrow(2, 0, H);
+  const c10::cuda::CUDAGuard guard(qkv.device());
+  const long long st[3] = {qkv.stride(0), qkv.stride(1), qkv.stride(2)};
+  raise(b200awq_rope_kv_store(qkv.data_ptr(), freqs.data_ptr<float>(), k_cache.data_ptr(), v_cache.data_ptr(), layout, (int)B,
+                              (int)S, (int)H, kv_heads, (int)D, (int)max_len, (int)start_pos, st, dt, current_stream()));
+  return qkv.narrow(2, 0, H);
 }
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -590,6 +634,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         "Attention of a chunk of queries over a KV cache in either of tinychat's layouts, read in place", py::arg("q"),
         py::arg("k_cache"), py::arg("v_cache"), py::arg("seqlen_k"), py::arg("softmax_scale") = py::none(),
         py::arg("causal") = true);
+  m.def("rope_kv_store", &rope_kv_store,
+        "RoPE of a chunk's q and k in the fused qkv output with the store of k and v into a KV cache, one launch",
+        py::arg("qkv"), py::arg("freqs"), py::arg("k_cache"), py::arg("v_cache"), py::arg("start_pos"));
   m.def("set_pdl", [](bool on) { return b200awq_set_pdl(on ? 1 : 0) != 0; }, "programmatic dependent launch on/off");
   m.def("launch_count", []() { return b200awq_launch_count(); }, "kernels launched by libb200awq so far");
   m.def("version", []() { return std::string(b200awq_version()); });

@@ -148,6 +148,11 @@ int launch_rope_with_pos(const void* x, const float* freqs, void* y, int s, int 
 int launch_rope_neox(const long long* positions, void* query, void* key, const void* cos_sin, int tokens, int q_heads,
                      int k_heads, int head_size, int rot_dim, long long q_stride, long long k_stride, int dtype, bool pdl,
                      cudaStream_t stream);
+// RoPE of a chunk's q / k in the fused qkv output with the store of k / v into a KV cache; arguments as
+// b200awq_rope_kv_store, validated (rope_kv_store.cu)
+int launch_rope_kv_store(void* qkv, const float* freqs, void* k_cache, void* v_cache, int layout, int batch, int seqlen,
+                         int heads, int kv_heads, int head_dim, int max_len, int start_pos, const long long* qkv_strides,
+                         int dtype, bool pdl, cudaStream_t stream);
 
 // forward attention over many queries, D in {64, 72, 128}; arguments as b200awq_prefill_attention (prefill_attention.cu)
 int launch_prefill_attention(const void* q, const void* k, const void* v, void* out, const int* cu_q, const int* cu_k, int batch,

@@ -55,6 +55,8 @@ def lib() -> ctypes.CDLL:
         L.b200awq_kv_cache_attention.restype = ci
         L.b200awq_kv_cache_attention_workspace_bytes.argtypes = [ci, ci, ci, ci, ci, ci, ci]
         L.b200awq_kv_cache_attention_workspace_bytes.restype = sz
+        L.b200awq_rope_kv_store.argtypes = [vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, ci, vp, ci, vp]
+        L.b200awq_rope_kv_store.restype = ci
         L.b200awq_rope_with_pos.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, vp, vp, ci, vp]
         L.b200awq_rope_with_pos.restype = ci
         L.b200awq_rotary_embedding_neox.argtypes = [vp, vp, vp, vp, ci, ci, ci, ci, ci, ctypes.c_longlong, ctypes.c_longlong, ci, vp]
