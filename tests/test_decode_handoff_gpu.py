@@ -1,7 +1,10 @@
 """The one-token decode kernel's per-SM handoff (DESIGN §3.1) changes only when weight copies are issued, never what is
 computed.  Every case runs Llama-3-8B-shaped decode launches (qkv 6144 x 4096, o 4096 x 4096, gate / up 14336 x 4096,
 down 4096 x 14336: every plan, including the k-split one) with programmatic dependent launch on, and compares the
-outputs bit for bit with the same launches run with it off, where no two launches of a stream overlap:
+outputs bit for bit with the same launches run with it off, where no two launches of a stream overlap.  Each case runs
+twice: with gate and up as two plain GEMVs, and with the fused MLP front half (b200awq_w4a16_mlp_front: gate, up and
+SiLU * mul in one decode launch, w4a16_decode_kernel<true, false>) between the second RMSNorm and down, the decode step
+tinychat runs:
   * the decode step captured in a CUDA graph and replayed many times;
   * decode right after RMSNorm and right after decode attention;
   * two streams running decode chains at once (the counters then also count the other stream's producers);
@@ -19,6 +22,9 @@ DEV = "cuda:0"
 DT = torch.float16
 HID, INTER = 4096, 14336
 SHAPES = {"qkv": (HID, 6144), "o": (HID, HID), "gate": (HID, INTER), "up": (HID, INTER), "down": (INTER, HID)}
+MLP = ("gemv", "fused")   # gate and up as two GEMVs, or the fused MLP front half
+# the outputs each layer keeps: the fused MLP front writes silu(gate) * up in place of the two products
+OUTS = {"gemv": ("qkv", "o", "gate", "up", "down"), "fused": ("qkv", "o", "act", "down")}
 
 
 def _p(t):
@@ -35,6 +41,13 @@ def _gemv(x, w, y):
     assert rc == 0, P.lib().b200awq_strerror(rc)
 
 
+def _mlp_front(x, gate, up, y):
+    """One fp16 token: the fused kernel, which needs no workspace."""
+    rc = P.lib().b200awq_w4a16_mlp_front(_p(x), *map(_p, gate), *map(_p, up), _p(y), 1, y.shape[-1], x.shape[-1], 128, 0,
+                                         None, 0, _st())
+    assert rc == 0, P.lib().b200awq_strerror(rc)
+
+
 def _rmsnorm(x, g, y):
     rc = P.lib().b200awq_rmsnorm(_p(x), _p(g), _p(y), 1, x.shape[-1], 1e-5, 0, _st())
     assert rc == 0, P.lib().b200awq_strerror(rc)
@@ -42,14 +55,17 @@ def _rmsnorm(x, g, y):
 
 class Model:
     """`layers` decoder layers of linears (distinct weights) with RMSNorm between them, so that values stay in range:
-    qkv after RMSNorm, o after qkv (decode after decode), gate after RMSNorm, up after gate, down after RMSNorm."""
+    qkv after RMSNorm, o after qkv (decode after decode), then with mlp = "gemv" gate after RMSNorm and up after gate,
+    with mlp = "fused" the MLP front after RMSNorm; down after RMSNorm."""
 
-    def __init__(self, layers, seed):
+    def __init__(self, layers, seed, mlp="gemv"):
+        self.mlp = mlp
         self.w = [{n: gen_layer(N, K, DT, seed=seed + 10 * l + i, device=DEV) for i, (n, (K, N)) in enumerate(SHAPES.items())}
                   for l in range(layers)]
         self.g = {n: (1.0 + 0.1 * gen_x(1, n, DT, seed=seed + n, device=DEV)).view(n) for n in (HID, INTER)}
         self.h0 = gen_x(1, HID, DT, seed=seed + 1, device=DEV)
-        self.bufs = [{n: torch.empty(1, SHAPES[n][1], dtype=DT, device=DEV) for n in SHAPES} for _ in self.w]
+        width = {n: N for n, (K, N) in SHAPES.items()} | {"act": INTER}
+        self.bufs = [{n: torch.empty(1, width[n], dtype=DT, device=DEV) for n in OUTS[mlp]} for _ in self.w]
         self.norm = [{k: torch.empty(1, n, dtype=DT, device=DEV) for k, n in (("a", HID), ("m", HID), ("d", INTER))}
                      for _ in self.w]
 
@@ -60,14 +76,17 @@ class Model:
             _gemv(nb["a"], w["qkv"], b["qkv"])
             _gemv(nb["a"], w["o"], b["o"])
             _rmsnorm(b["o"], self.g[HID], nb["m"])
-            _gemv(nb["m"], w["gate"], b["gate"])
-            _gemv(nb["m"], w["up"], b["up"])
-            _rmsnorm(b["up"], self.g[INTER], nb["d"])
+            if self.mlp == "fused":
+                _mlp_front(nb["m"], w["gate"], w["up"], b["act"])
+            else:
+                _gemv(nb["m"], w["gate"], b["gate"])
+                _gemv(nb["m"], w["up"], b["up"])
+            _rmsnorm(b["act" if self.mlp == "fused" else "up"], self.g[INTER], nb["d"])
             _gemv(nb["d"], w["down"], b["down"])
             h = b["down"]
 
-    def outputs(self):
-        return [t.clone() for b in self.bufs for t in b.values()]
+    def outputs(self, names=None):
+        return [t.clone() for b in self.bufs for n, t in b.items() if names is None or n in names]
 
     def clear(self):
         for b in self.bufs:
@@ -92,7 +111,12 @@ def _same(a, b):
 
 
 def test_step_graph_replayed_matches_pdl_off():
-    m = Model(4, seed=100)
+    for mlp in MLP:
+        _step_graph_replayed(mlp)
+
+
+def _step_graph_replayed(mlp):
+    m = Model(4, seed=100, mlp=mlp)
     _pdl_off(m.run)
     want = m.outputs()
     side = torch.cuda.Stream()
@@ -111,9 +135,14 @@ def test_step_graph_replayed_matches_pdl_off():
 
 
 def test_decode_after_attention_matches_pdl_off():
-    """o right after decode attention, then the rest of the layer."""
+    """o, and gate or the fused MLP front, right after decode attention."""
+    for mlp in MLP:
+        _decode_after_attention(mlp)
+
+
+def _decode_after_attention(mlp):
     eng = P.engine()
-    m = Model(2, seed=200)
+    m = Model(2, seed=200, mlp=mlp)
     B, H, Hkv, D, L, t = 1, 32, 8, 128, 512, 300
     gq = torch.Generator().manual_seed(7)
     qkv = torch.randn(B, 1, H + 2 * Hkv, D, generator=gq).to(DT).to(DEV)
@@ -127,22 +156,30 @@ def test_decode_after_attention_matches_pdl_off():
             att = eng.single_query_attention(qkv[:, 0, :H], qkv[:, 0, H:H + Hkv], qkv[:, 0, H + Hkv:], kc, vc, None, None,
                                              t, D, 500000.0, 1.0, True)
             _gemv(att.reshape(1, H * D), w["o"], b["o"])
-            _gemv(att.reshape(1, H * D), w["gate"], b["gate"])
+            if mlp == "fused":
+                _mlp_front(att.reshape(1, H * D), w["gate"], w["up"], b["act"])
+            else:
+                _gemv(att.reshape(1, H * D), w["gate"], b["gate"])
             outs.append(att)
         return outs
 
+    names = ("o", "act" if mlp == "fused" else "gate")
     _pdl_off(run)
-    want = m.outputs()
+    want = m.outputs(names)
     for _ in range(5):
         m.clear()
         run()
         torch.cuda.synchronize()
-        got = m.outputs()
-        _same([want[i] for i in range(len(want)) if i % 5 in (1, 2)], [got[i] for i in range(len(got)) if i % 5 in (1, 2)])
+        _same(want, m.outputs(names))
 
 
 def test_two_streams_of_decode_chains_match_pdl_off():
-    a, b = Model(3, seed=300), Model(3, seed=400)
+    for mlp in MLP:
+        _two_streams(mlp)
+
+
+def _two_streams(mlp):
+    a, b = Model(3, seed=300, mlp=mlp), Model(3, seed=400, mlp=mlp)
     _pdl_off(a.run)
     _pdl_off(b.run)
     want_a, want_b = a.outputs(), b.outputs()
@@ -162,7 +199,12 @@ def test_two_streams_of_decode_chains_match_pdl_off():
 
 
 def test_decode_chain_beside_a_long_kernel_matches_pdl_off():
-    m = Model(4, seed=500)
+    for mlp in MLP:
+        _beside_a_long_kernel(mlp)
+
+
+def _beside_a_long_kernel(mlp):
+    m = Model(4, seed=500, mlp=mlp)
     _pdl_off(m.run)
     want = m.outputs()
     big = torch.randn(8192, 8192, device=DEV, dtype=DT)

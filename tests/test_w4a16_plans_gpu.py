@@ -76,8 +76,9 @@ def check_plan_output(m, n, k, dtype, entry, what, layer=None):
 
 
 # ------------------------------------------------------------------------------------------------ plans pinned
-# Child process: for each case [m, n, k, dtype, entry], (name, grid, shared memory) of every kernel of one call, read
-# from the exported Chrome trace, after a first call outside the profiled region (module load, descriptors).
+# Child process: for each case [m, n, k, dtype, entry], (name, grid, shared memory) of every kernel of one call in launch
+# order, read from the exported Chrome trace, after a first call outside the profiled region (module load, descriptors).
+# Entry "mlp_front" is b200awq_w4a16_mlp_front with both weight sets and a workspace.
 _PROFILE = """
 import ctypes, json, os, sys, tempfile
 sys.path[:0] = sys.argv[1:3]
@@ -95,7 +96,12 @@ for m, n, k, dt, entry in json.loads(sys.argv[3]):
     y = torch.empty(m, n, dtype=dtype, device="cuda")
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     code = 0 if dt == "f16" else 1
-    if entry == "gemv":
+    if entry == "mlp_front":
+        qw2, s2, z2 = torch.zeros_like(qw), torch.zeros_like(s), torch.zeros_like(z)
+        nb = L.b200awq_w4a16_mlp_front_workspace_bytes(m, n, k)
+        ws = torch.empty(nb, dtype=torch.uint8, device="cuda")
+        run = lambda: L.b200awq_w4a16_mlp_front(x.data_ptr(), qw.data_ptr(), s.data_ptr(), z.data_ptr(), qw2.data_ptr(), s2.data_ptr(), z2.data_ptr(), y.data_ptr(), m, n, k, 128, code, ws.data_ptr(), nb, st)
+    elif entry == "gemv":
         run = lambda: L.b200awq_w4a16_gemv(x.data_ptr(), qw.data_ptr(), s.data_ptr(), z.data_ptr(), y.data_ptr(), m, n, k, 128, code, st)
     else:
         run = lambda: L.b200awq_w4a16_gemm(x.data_ptr(), qw.data_ptr(), s.data_ptr(), z.data_ptr(), y.data_ptr(), m, n, k, 128, code, None, 0, st)
@@ -114,7 +120,7 @@ for m, n, k, dt, entry in json.loads(sys.argv[3]):
         finally:
             os.unlink(path)
         kernels = [[e["name"], e.get("args", {}).get("grid"), e.get("args", {}).get("shared memory")]
-                   for e in events if e.get("cat") == "kernel"]
+                   for e in sorted((e for e in events if e.get("cat") == "kernel"), key=lambda e: e.get("ts", 0))]
         if kernels:
             break
     out.append(kernels)

@@ -9,7 +9,11 @@ test_w4a16_plans_gpu.py, and the hand-worked values in test_w4a16_plans_cpu.py m
 
 `edge_cases(sms)` derives the GPU cases from the SM count: shapes whose partition over the SMs is ragged, k splits
 that leave odd group counts, every plan class the dispatch can reach, and the token counts at route boundaries.
-`SERVED` lists the projections of the models the project serves."""
+`SERVED` lists the projections of the models the project serves.
+
+`mlp_front_plan(m, n, k, dtype, sms)` mirrors b200awq_w4a16_mlp_front: the fused one-token kernel (launch_decode_impl
+with two weight sets), else the two kMlpProjection products and silu_mul_kernel; `mlp_front_cases(sms)` derives its
+GPU cases (test_mlp_front_plans_gpu.py)."""
 import functools
 from dataclasses import dataclass, field, replace
 
@@ -44,8 +48,9 @@ def _align(v, a):
 
 @dataclass(frozen=True)
 class Plan:
-    route: str           # decode, ring, flat, stream, tile
-    kernel: str          # as the profiler tests report it: w4a16_<route>_kernel, w4a16_wgmma_kernel<TN>
+    route: str           # decode, ring, flat, stream, tile; fused (the MLP front's decode kernel), silu_mul
+    kernel: str          # as the profiler tests report it: w4a16_<route>_kernel, w4a16_wgmma_kernel<TN>,
+                         # w4a16_decode_kernel<true, false> (fused), silu_mul_kernel
     grid: int            # CTAs of the launch
     smem: int            # dynamic shared memory of the launch, bytes
     S: int = 1           # k split: CTAs per cluster
@@ -72,8 +77,8 @@ class Plan:
     @property
     def klass(self):
         """The plan class: what decides which code of the kernel runs (instantiation, split, partition loop)."""
-        if self.route == "decode":
-            return ("decode", self.S)
+        if self.route in ("decode", "fused"):
+            return (self.route, self.S)
         if self.route == "ring":
             return ("ring", self.S, self.Mp)
         if self.route == "stream":
@@ -84,8 +89,10 @@ class Plan:
 
 
 # ------------------------------------------------------------------------------------------------ launchers
-def decode_plan(n, k, sms):
-    """launch_decode_impl (no override): None where it returns B200AWQ_ERR_SHAPE."""
+def decode_plan(n, k, sms, nt=1):
+    """launch_decode_impl (no override): None where it returns B200AWQ_ERR_SHAPE.  `nt` weight sets: 2 for the fused
+    MLP front (w4a16_decode_kernel<true, false>), whose red and exchange regions hold 16 nt floats per row block; the
+    split does not depend on it."""
     G, Q = k // GROUP, n // 4
 
     def eff(s):
@@ -107,12 +114,13 @@ def decode_plan(n, k, sms):
         return None
     ngr = -(-G // S)
     off = _align(8 * (2 * DEC_MAX_SLOTS + 2 * DEC_RED + 1 + nrb_max), 128)
-    off += ngr * DEC_GROUP_BYTES + ngr * 16 + min(DEC_RED, nrb_max) * DEC_CONS * 16 * 4 + S * nrb_max * 16 * 4
+    off += ngr * DEC_GROUP_BYTES + ngr * 16 + min(DEC_RED, nrb_max) * DEC_CONS * 16 * nt * 4 + S * nrb_max * 16 * nt * 4
     off = _align(off, 128)
     ns = min((DEC_BUDGET - off) // DEC_SLOT_BYTES, DEC_MAX_SLOTS)
     if ns < 3:
         return None
-    return Plan("decode", "w4a16_decode_kernel", units * S, off + ns * DEC_SLOT_BYTES, S=S, units=units,
+    route, kernel = ("fused", "w4a16_decode_kernel<true, false>") if nt == 2 else ("decode", "w4a16_decode_kernel")
+    return Plan(route, kernel, units * S, off + ns * DEC_SLOT_BYTES, S=S, units=units,
                 per_unit=(Q // units, -(-Q // units)), ns=ns)
 
 
@@ -231,9 +239,10 @@ class Rejected(ValueError):
 
 @functools.lru_cache(maxsize=None)
 def plan(m, n, k, dtype, entry, sms):
-    """The plan the entry `entry` ("gemv", "gemm" or "linear") launches for x [m, k], W [n, k] of `dtype` ("f16" or
-    "bf16") on a device with `sms` SMs (api.cu launch_w4a16).  Raises Rejected where the entry returns an error."""
-    assert dtype in ("f16", "bf16") and entry in ("gemv", "gemm", "linear")
+    """The plan the entry `entry` ("gemv", "gemm" or "linear"; "mlp": one projection of b200awq_w4a16_mlp_front's
+    composed path, the kMlpProjection envelope) launches for x [m, k], W [n, k] of `dtype` ("f16" or "bf16") on a device
+    with `sms` SMs (api.cu launch_w4a16).  Raises Rejected where the entry returns an error."""
+    assert dtype in ("f16", "bf16") and entry in ("gemv", "gemm", "linear", "mlp")
     if m < 1 or n < 8 or k < GROUP or n % 8 or k % GROUP:
         raise Rejected("shape")
     if entry == "gemv" and m > 7:
@@ -241,7 +250,8 @@ def plan(m, n, k, dtype, entry, sms):
     if entry != "gemv" and n % BM and (entry == "gemm" or m >= 8):
         raise Rejected("shape")
     env = "gemv" if entry == "gemv" or (entry == "linear" and m < 8) else "gemm"
-    big_mid = env == "gemm" and m > 8 and n * k >= BIG_MID_WEIGHTS
+    # kMlpProjection is kGemm without the big-layer rule
+    big_mid = env == "gemm" and entry != "mlp" and m > 8 and n * k >= BIG_MID_WEIGHTS
     failed = []
     if not big_mid:
         if m == 1 and dtype == "f16":
@@ -505,14 +515,113 @@ def edge_cases(sms):
             + _boundary_cases(sms))
 
 
+# ------------------------------------------------------------------------------------------------ MLP front half
+def silu_mul_plan(count, sms, vec=True):
+    """launch_silu_mul over `count` elements of one flat row: 256 threads, 8 elements per thread when every pointer is
+    16-byte aligned, grid-stride over at most 8 CTAs per SM."""
+    return Plan("silu_mul", "silu_mul_kernel", max(1, min(-(-(count // 8 if vec else count) // 256), 8 * sms)), 0)
+
+
+@functools.lru_cache(maxsize=None)
+def mlp_front_plan(m, n, k, dtype, sms, y_aligned=True):
+    """The launches of one b200awq_w4a16_mlp_front call, in stream order: the fused one-token kernel (one fp16 token,
+    when its ring gets >= 3 slots), else gate and up through the kMlpProjection envelope into the workspace, then
+    silu_mul_kernel over the m n products (vectorised when y is 16-byte aligned: the workspace always is).  Raises
+    Rejected where the entry returns an error."""
+    if m < 1 or n < 8 or k < GROUP or n % 8 or k % GROUP or (m >= 8 and n % BM):
+        raise Rejected("shape")
+    if m == 1 and dtype == "f16":
+        p = decode_plan(n, k, sms, nt=2)
+        if p:
+            return (p,)
+    proj = plan(m, n, k, dtype, "mlp", sms)
+    return (proj, proj, silu_mul_plan(m * n, sms, y_aligned))
+
+
+def _fused_candidates(sms):
+    """(n, k) for k <= 32768 and, for every cluster count and row-block count r, the fewest even quad rows that give a
+    CTA r row blocks and the most that do: the shapes at which the decode kernel's shared-memory layout changes."""
+    qs = {2, 4}
+    for S in (1, 2, 4, 8):
+        if sms % S:
+            continue
+        u = sms // S
+        for r in range(1, DEC_MAX_RB + 1):
+            lo = 4 * u * (r - 1) + 1
+            qs.update((lo + lo % 2, 4 * u * r))
+    return [(4 * q, k) for k in _ks() for q in sorted(qs)]
+
+
+@functools.lru_cache(maxsize=None)
+def fused_reach(sms):
+    """Over _fused_candidates: ({split: smallest (n, k)}, {ring slots: smallest-weight (n, k)}) of the fused kernel, and
+    the smallest-weight (n, k) it declines while the plain decode kernel takes it."""
+    splits, depths, decline = {}, {}, None
+    for n, k in _fused_candidates(sms):
+        p = decode_plan(n, k, sms, nt=2)
+        if p is None:
+            if decode_plan(n, k, sms) and (decline is None or n * k < decline[0] * decline[1]):
+                decline = (n, k)
+            continue
+        for d, key in ((splits, p.S), (depths, p.ns)):
+            if key not in d or n * k < d[key][0] * d[key][1]:
+                d[key] = (n, k)
+    return splits, depths, decline
+
+
+def mlp_front_cases(sms):
+    """The GPU cases of b200awq_w4a16_mlp_front on a device with `sms` SMs (entry "mlp_front"; `expect` holds attributes
+    of the call's first launch):
+      * fused: each split the fused kernel reaches, at Q = 4 units j -+ 2 quad rows (j = 1, 2: two units get one quad
+        row fewer or more than the rest), the smallest k of that split, preferring an odd or uneven group count per rank;
+      * fused: the smallest-weight shape of every ring depth it reaches;
+      * the smallest shape the fused kernel declines (fewer than 3 ring slots) and the plain decode kernel takes: two
+        plain decode launches and silu_mul;
+      * the gate / up shapes of the Llama models in SERVED (make_fused_mlp replaces LlamaMLP only), one fp16 token;
+      * composed on Llama-3-8B gate / up at m = 1 (bf16), 2 .. 17 tokens across every route boundary, among them 9..16
+        tokens on this 58.7 M-weight layer, where kMlpProjection takes the flat launch and the GEMM the tile launch; a
+        partial wgmma token tile; and 6 tokens with n % 128 != 0 (stream kernel)."""
+    out = []
+    splits, depths, decline = fused_reach(sms)
+    for S in sorted(splits):
+        units = sms // S
+        for j in (1, 2):
+            for dq in (-2, 2):
+                Q = 4 * units * j + dq
+                hits = [k for k in _ks() if (p := decode_plan(4 * Q, k, sms, nt=2)) and p.S == S]
+                odd = [k for k in hits if k // GROUP // S > DEC_PIECE and ((k // GROUP) % S or (k // GROUP // S) % 2)]
+                if not hits:
+                    continue
+                lo, hi = (4 * j - 1, 4 * j) if dq < 0 else (4 * j, 4 * j + 1)
+                out.append(_case(f"fused_S{S}_q{4 * j}{dq:+d}", 1, 4 * Q, (odd or hits)[0], "f16", "mlp_front",
+                                 route="fused", S=S, units=units, per_unit=(lo, hi)))
+    for ns, (n, k) in sorted(depths.items()):
+        out.append(_case(f"fused_ns{ns}", 1, n, k, "f16", "mlp_front", route="fused", ns=ns))
+    if decline:
+        n, k = decline
+        out.append(_case("fused_declines", 1, n, k, "f16", "mlp_front", route="decode"))
+    for model in ("llama2_7b", "llama3_8b", "llama2_70b_tp8"):
+        n, k = next((n, k) for name, n, k in SERVED[model] if name == "gate_up")
+        out.append(_case(f"{model}_gate_up", 1, n, k, "f16", "mlp_front", route="fused"))
+    n, k = next((n, k) for name, n, k in SERVED["llama3_8b"] if name == "gate_up")
+    for i, m in enumerate((1, 2, 4, 5, 7, 8, 9, 12, 16, 17)):
+        dtype = "bf16" if m == 1 else ("f16", "bf16")[i % 2]
+        out.append(_case(f"composed_m{m}", m, n, k, dtype, "mlp_front", route=plan(m, n, k, dtype, "mlp", sms).route))
+    m = next(m for m in range(18, 4097) if (p := plan(m, n, k, "bf16", "mlp", sms)).route == "tile" and m % p.tn
+             and m // p.tn >= 1)
+    out.append(_case("composed_partial_tile", m, n, k, "bf16", "mlp_front", route="tile"))
+    out.append(_case("composed_stream_n_not_128", 6, 2056, k, "f16", "mlp_front", route="stream"))
+    return out
+
+
 # ------------------------------------------------------------------------------------------------ sampled outputs
 def edge_channels(p, n):
     """Output channels that carry the plan's edges: the first and last row block (decode) or octet (ring) of every
     unit, the first and last CTA row block (stream), the first and last channel of every 128-channel tile and the
     channels where a tile's warps and warpgroups meet (flat / tile); always the first and last channel."""
     ch = {0, n - 1}
-    if p.route in ("decode", "ring"):
-        size, block = (4, 16) if p.route == "decode" else (8, 8)
+    if p.route in ("decode", "fused", "ring"):
+        size, block = (8, 8) if p.route == "ring" else (4, 16)
         rows = n // size
         for u in range(p.units):
             lo, hi = u * rows // p.units * size, (u + 1) * rows // p.units * size
