@@ -267,6 +267,35 @@ int b200awq_rope_kv_store(void* qkv, const float* freqs, void* k_cache, void* v_
                           int heads, int kv_heads, int head_dim, int max_len, int start_pos,
                           const long long qkv_strides[3], int dtype, void* stream);
 
+/* The choice of the next token from fp32 logits, in one launch: what tinychat's per-token block computes
+ * (tinychat/stream_generators/stream_gen.py: TemperatureLogitsWarper, RepetitionPenaltyLogitsProcessor,
+ * TopPLogitsWarper, TopKLogitsWarper, then argmax or softmax + torch.multinomial).  For each row b < batch, with x the
+ * row's vocab logits (logits + b * logits_row_stride; rows may alias, e.g. a stride of 0):
+ *   1. temperature != 1: x = x / temperature (an fp32 division);
+ *   2. repetition_penalty > 1: every DISTINCT id of prev_ids[b * prev_row_stride + i], i < n_prev, that lies in
+ *      [0, vocab) becomes x < 0 ? x * penalty : x / penalty (ids outside are ignored);
+ *   3. 0 < top_p < 1: in ascending order of (x, index) -- a stable sort -- tokens whose inclusive cumulative softmax
+ *      probability is <= fp32(1 - top_p) are removed; the last token in that order is always kept;
+ *   4. 0 < top_k < vocab: tokens below the top_k-th largest value left after 3 are removed (ties at it are kept);
+ *   5. greedy != 0: the token is the smallest index among the maxima of the kept tokens (uniforms may be NULL);
+ *      otherwise, with u = uniforms[b] in [0, 1) and p_i = exp(x_i - max) over the kept tokens, the smallest index i
+ *      whose cumulative kept mass through i (in index order) exceeds u * sum p -- the inverse CDF;
+ *   6. tokens[b] = that index (int64).
+ * Probabilities are fp32 exp(x - max) in 2^-44 fixed point, summed exactly: the top-p rule may decide differently from
+ * float64 arithmetic only for tokens whose cumulative probability lies within 1e-5 of 1 - top_p (DESIGN §3.12).  NaN
+ * logits count as -inf; -inf entries of a row with a finite maximum are never drawn; every row, even an all -inf or NaN
+ * one, gets an id in [0, vocab).
+ * B200AWQ_ERR_SHAPE: batch < 0, vocab < 1 or > B200AWQ_SAMPLE_MAX_VOCAB, n_prev < 0, temperature not finite or <= 0,
+ * repetition_penalty not finite or < 1, top_p outside (0, 1] (1 = off), top_k < 0 (0 = off).  B200AWQ_ERR_ALIGN: logits
+ * or tokens NULL or misaligned, uniforms when !greedy, prev_ids when n_prev > 0 and repetition_penalty > 1 (4-, 8-, 4-
+ * and 8-byte alignment).  batch == 0 is a no-op.  One launch, no workspace, no global atomics, deterministic, safe under
+ * graph capture; logits, prev_ids and uniforms are read after the launch's dependency wait. */
+#define B200AWQ_SAMPLE_MAX_VOCAB 262144
+int b200awq_sample_next_token(const float* logits, long long logits_row_stride, int batch, int vocab,
+                              const long long* prev_ids, long long prev_row_stride, int n_prev, float temperature,
+                              float repetition_penalty, float top_p, int top_k, int greedy, const float* uniforms,
+                              long long* tokens, void* stream);
+
 /* ---- W8A8 (int8 weights, int8 per-token activations): the vision-tower ops of the reference's extension
  * (csrc/pybind.cpp:30-37), called by awq/quantize/w8a8_linear.py and tinychat's QuantSiglipEncoder /
  * QuantInternVisionEncoder.  Scales are fp16 everywhere (the reference reads them as at::Half).  fp32 activations,

@@ -337,6 +337,25 @@ int b200awq_rope_kv_store(void* qkv, const float* freqs, void* k_cache, void* v_
                                                static_cast<cudaStream_t>(stream)));
 }
 
+int b200awq_sample_next_token(const float* logits, long long logits_row_stride, int batch, int vocab,
+                              const long long* prev_ids, long long prev_row_stride, int n_prev, float temperature,
+                              float repetition_penalty, float top_p, int top_k, int greedy, const float* uniforms,
+                              long long* tokens, void* stream) {
+  if (batch < 0 || vocab < 1 || vocab > B200AWQ_SAMPLE_MAX_VOCAB || n_prev < 0 ||
+      !(std::isfinite(temperature) && temperature > 0.f) ||
+      !(std::isfinite(repetition_penalty) && repetition_penalty >= 1.f) || !(top_p > 0.f && top_p <= 1.f) || top_k < 0)
+    return B200AWQ_ERR_SHAPE;
+  auto aligned = [](const void* p, uintptr_t bytes) { return p && (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; };
+  if (!aligned(logits, 4) || !aligned(tokens, 8) || (!greedy && !aligned(uniforms, 4)) ||
+      (n_prev > 0 && repetition_penalty > 1.f && !aligned(prev_ids, 8)))
+    return B200AWQ_ERR_ALIGN;
+  if (batch == 0) return 0;
+  if (int e = check_device()) return e;
+  return counted(b200awq::launch_sample_next_token(logits, logits_row_stride, batch, vocab, prev_ids, prev_row_stride, n_prev,
+                                                   temperature, repetition_penalty, top_p, top_k, greedy, uniforms, tokens,
+                                                   pdl_enabled(), static_cast<cudaStream_t>(stream)));
+}
+
 int b200awq_rope_with_pos(const void* x, const float* freqs, void* y, int s, int b, int h, int d, int d2,
                           const long long in_strides[4], const long long out_strides[4], int dtype, void* stream) {
   if (int e = check_dtype(dtype)) return e;

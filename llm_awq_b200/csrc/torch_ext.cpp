@@ -598,6 +598,49 @@ torch::Tensor rope_kv_store(const torch::Tensor& qkv, const torch::Tensor& freqs
   return qkv.narrow(2, 0, H);
 }
 
+// The next token of each row, one launch (include/b200awq.h, b200awq_sample_next_token).  logits fp32 [B, V] with a
+// contiguous last dimension (tinychat's logits[:, -1, :] view is read in place); prev_ids int64 [B, n] with a contiguous
+// last dimension, or None; uniforms fp32 [B] in [0, 1), required unless greedy.  Returns int64 [B] on logits' device.
+torch::Tensor sample_next_token(const torch::Tensor& logits, c10::optional<torch::Tensor> prev_ids, double temperature,
+                                double repetition_penalty, double top_p, int64_t top_k, bool greedy,
+                                c10::optional<torch::Tensor> uniforms) {
+  const char* fn = "sample_next_token";
+  TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == at::ScalarType::Float && logits.dim() == 2 &&
+                  logits.stride(1) == 1,
+              fn, ": logits must be a float32 CUDA tensor [batch, vocab] with a contiguous last dimension");
+  const int64_t B = logits.size(0), V = logits.size(1);
+  TORCH_CHECK(B <= INT32_MAX && V <= INT32_MAX && top_k >= 0 && top_k <= INT32_MAX, fn, ": sizes out of range");
+  const long long* ids = nullptr;
+  long long ids_stride = 0;
+  int n_prev = 0;
+  if (prev_ids.has_value()) {
+    const torch::Tensor& p = prev_ids.value();
+    TORCH_CHECK(p.device() == logits.device() && p.scalar_type() == at::ScalarType::Long && p.dim() == 2 &&
+                    p.size(0) == B && (p.stride(1) == 1 || p.size(1) <= 1) && p.size(1) <= INT32_MAX,
+                fn, ": prev_ids must be an int64 tensor [batch, n] on logits' device with a contiguous last dimension");
+    ids = reinterpret_cast<const long long*>(p.data_ptr<int64_t>());
+    ids_stride = p.stride(0);
+    n_prev = (int)p.size(1);
+  }
+  const float* u = nullptr;
+  if (uniforms.has_value()) {
+    const torch::Tensor& t = uniforms.value();
+    TORCH_CHECK(t.device() == logits.device() && t.scalar_type() == at::ScalarType::Float && t.dim() == 1 &&
+                    t.numel() == B && t.is_contiguous(),
+                fn, ": uniforms must be a contiguous float32 tensor [batch] on logits' device");
+    u = t.data_ptr<float>();
+  }
+  TORCH_CHECK(greedy || u, fn, ": uniforms are required unless greedy");
+  const c10::cuda::CUDAGuard guard(logits.device());
+  torch::Tensor tokens = torch::empty({B}, logits.options().dtype(torch::kInt64));
+  if (B == 0) return tokens;
+  raise(b200awq_sample_next_token(logits.data_ptr<float>(), (long long)logits.stride(0), (int)B, (int)V, ids, ids_stride,
+                                  n_prev, (float)temperature, (float)repetition_penalty, (float)top_p, (int)top_k,
+                                  greedy ? 1 : 0, u, reinterpret_cast<long long*>(tokens.data_ptr<int64_t>()),
+                                  current_stream()));
+  return tokens;
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "H100 (sm_90a) drop-in for llm-awq's awq_inference_engine (W4A16 and W8A8 paths)";
   m.def("gemm_forward_cuda_new", &gemm_forward_cuda_new, "New quantized GEMM kernel.");
@@ -637,7 +680,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("rope_kv_store", &rope_kv_store,
         "RoPE of a chunk's q and k in the fused qkv output with the store of k and v into a KV cache, one launch",
         py::arg("qkv"), py::arg("freqs"), py::arg("k_cache"), py::arg("v_cache"), py::arg("start_pos"));
-  m.def("set_pdl", [](bool on) { return b200awq_set_pdl(on ? 1 : 0) != 0; }, "programmatic dependent launch on/off");
+  m.def("sample_next_token", &sample_next_token,
+        "tinychat's temperature, repetition penalty, top-p, top-k and the choice of the next token, one launch",
+        py::arg("logits"), py::arg("prev_ids"), py::arg("temperature"), py::arg("repetition_penalty"), py::arg("top_p"),
+        py::arg("top_k"), py::arg("greedy"), py::arg("uniforms") = py::none());
+  m.def("set_pdl",[](bool on) { return b200awq_set_pdl(on ? 1 : 0) != 0; }, "programmatic dependent launch on/off");
   m.def("launch_count", []() { return b200awq_launch_count(); }, "kernels launched by libb200awq so far");
   m.def("version", []() { return std::string(b200awq_version()); });
 }

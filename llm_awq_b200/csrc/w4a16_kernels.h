@@ -154,6 +154,12 @@ int launch_rope_kv_store(void* qkv, const float* freqs, void* k_cache, void* v_c
                          int heads, int kv_heads, int head_dim, int max_len, int start_pos, const long long* qkv_strides,
                          int dtype, bool pdl, cudaStream_t stream);
 
+// the next token from fp32 logits (temperature, repetition penalty, top-p, top-k, draw); arguments as
+// b200awq_sample_next_token, validated (sampling.cu)
+int launch_sample_next_token(const float* logits, long long logits_stride, int batch, int vocab, const long long* prev_ids,
+                             long long prev_stride, int n_prev, float temperature, float penalty, float top_p, int top_k,
+                             int greedy, const float* uniforms, long long* tokens, bool pdl, cudaStream_t stream);
+
 // forward attention over many queries, D in {64, 72, 128}; arguments as b200awq_prefill_attention (prefill_attention.cu)
 int launch_prefill_attention(const void* q, const void* k, const void* v, void* out, const int* cu_q, const int* cu_k, int batch,
                              int seqlen_q, int seqlen_k, int heads, int kv_heads, int head_dim, const long long* q_strides,
