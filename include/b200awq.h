@@ -46,7 +46,7 @@ extern "C" {
 #define B200AWQ_OK 0
 #define B200AWQ_ERR_SHAPE (-1)     /* n % 8 (gemv) / n % 128 (gemm), k % 128 (w8a8: k % 16), m out of range */
 #define B200AWQ_ERR_GROUP (-2)     /* group_size != 128 (reference: gemv_cuda.cu:289,332-335) */
-#define B200AWQ_ERR_ALIGN (-3)     /* a pointer is NULL or not 16-byte aligned */
+#define B200AWQ_ERR_ALIGN (-3)     /* a pointer is NULL or not 16-byte aligned (w8a8_linear: residual overlaps y) */
 #define B200AWQ_ERR_DTYPE (-4)     /* dtype is not F16 / BF16 (reference: dispatch_utils.cuh:7-18) */
 #define B200AWQ_ERR_BATCH (-5)     /* gemv with m outside 1..7 (reference: gemv_cuda.cu:291-330) */
 #define B200AWQ_ERR_WORKSPACE (-6) /* workspace smaller than b200awq_w4a16_gemm_workspace_bytes */
@@ -313,6 +313,23 @@ int b200awq_sample_next_token(const float* logits, long long logits_row_stride, 
  * m >= 1, n % 8 == 0, k % 16 == 0 (any k tail is exact). */
 int b200awq_w8a8_gemm(const void* x, const void* w, const void* wscales, const void* ascales, const void* bias, void* y,
                       int m, int n, int k, void* stream);
+
+/* The W8A8 linear with the vision towers' layer scale and residual in the same launch:
+ *   v = the b200awq_w8a8_gemm formula above (with or without bias), unchanged
+ *   y0 = rn_f16(v)
+ *   y1 = layer_scale ? rn_f16(f32(y0) * f32(layer_scale[j])) : y0
+ *   y[i, j] = residual ? rn_f16(f32(residual[i, j]) + f32(y1)) : y1
+ * each operation in fp32 and rounded once: bit-identical to b200awq_w8a8_gemm followed by PyTorch's fp16 `out * ls`
+ * and then `residual + out` (tinychat's QuantInternVisionEncoderLayer: `residual + out * self.ls1`;
+ * QuantSiglipEncoderLayer: `residual + out`).  The arguments and their checks are b200awq_w8a8_gemm's; layer_scale
+ * [n] and residual [m, n] (row-major) are fp16 and 16-byte aligned, and any of bias, layer_scale and residual may be
+ * NULL.  With layer_scale and residual both NULL this launches exactly what b200awq_w8a8_gemm launches.  residual
+ * must not overlap y (B200AWQ_ERR_ALIGN): the residual stream is written out of place, since the encoders keep every
+ * layer's input.  layer_scale and residual are read only after the launch's dependency wait, so either may be written
+ * by the launch right before it in the stream.  Every argument error returns before the device is touched.  One
+ * launch, no workspace, deterministic. */
+int b200awq_w8a8_linear(const void* x, const void* w, const void* wscales, const void* ascales, const void* bias,
+                        const void* layer_scale, const void* residual, void* y, int m, int n, int k, void* stream);
 
 /* Per-token int8 quantisation: scales[i] = rn_f16(amax_i / 127), q[i, j] = cvt.rni.sat(x[i, j] * (127 / amax_i)),
  * amax_i = max_j |x[i, j]| (a zero row gives codes 0 and scale 0).  Replaces invoke_quant(out, input, scale),

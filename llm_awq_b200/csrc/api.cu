@@ -398,14 +398,37 @@ int b200awq_w4a16_gemm(const void* x, const void* qweight, const void* scales, c
 }
 
 // ---------------------------------------------------------------- W8A8
-int b200awq_w8a8_gemm(const void* x, const void* w, const void* wscales, const void* ascales, const void* bias, void* y,
-                      int m, int n, int k, void* stream) {
+namespace {
+// b200awq_w8a8_gemm's argument checks that need no device
+int check_w8a8_gemm(const void* x, const void* w, const void* wscales, const void* ascales, const void* bias, const void* y,
+                    int m, int n, int k) {
   if (m < 1 || n < 8 || k < 16 || n % 8 || k % 16) return B200AWQ_ERR_SHAPE;
   if (!aligned16(x) || !aligned16(w) || !aligned16(y) || !wscales || !ascales) return B200AWQ_ERR_ALIGN;
   if ((reinterpret_cast<uintptr_t>(wscales) | reinterpret_cast<uintptr_t>(ascales) | reinterpret_cast<uintptr_t>(bias)) & 1u)
     return B200AWQ_ERR_ALIGN;
+  return 0;
+}
+}  // namespace
+
+int b200awq_w8a8_gemm(const void* x, const void* w, const void* wscales, const void* ascales, const void* bias, void* y,
+                      int m, int n, int k, void* stream) {
+  if (int e = check_w8a8_gemm(x, w, wscales, ascales, bias, y, m, n, k)) return e;
   if (int e = check_device()) return e;
   return counted(b200awq::launch_w8a8_gemm(x, w, wscales, ascales, bias, y, m, n, k, pdl_enabled(), static_cast<cudaStream_t>(stream)));
+}
+
+int b200awq_w8a8_linear(const void* x, const void* w, const void* wscales, const void* ascales, const void* bias,
+                        const void* layer_scale, const void* residual, void* y, int m, int n, int k, void* stream) {
+  if (int e = check_w8a8_gemm(x, w, wscales, ascales, bias, y, m, n, k)) return e;
+  if ((layer_scale && !aligned16(layer_scale)) || (residual && !aligned16(residual))) return B200AWQ_ERR_ALIGN;
+  if (residual) {  // the residual is read and y written by different threads: the two must not share a byte
+    const uintptr_t r = reinterpret_cast<uintptr_t>(residual), o = reinterpret_cast<uintptr_t>(y);
+    const uintptr_t bytes = (uintptr_t)m * (uintptr_t)n * 2u;
+    if (r < o + bytes && o < r + bytes) return B200AWQ_ERR_ALIGN;
+  }
+  if (int e = check_device()) return e;
+  return counted(b200awq::launch_w8a8_gemm(x, w, wscales, ascales, bias, y, m, n, k, pdl_enabled(),
+                                           static_cast<cudaStream_t>(stream), layer_scale, residual));
 }
 
 namespace {
@@ -476,7 +499,7 @@ const char* b200awq_strerror(int code) {
     case B200AWQ_ERR_SHAPE:
       return "unsupported shape (need n % 8 == 0 [gemm: n % 128 == 0], k % 128 == 0 [w8a8 gemm: k % 16 == 0], m >= 1)";
     case B200AWQ_ERR_GROUP: return "unsupported group size (only 128)";
-    case B200AWQ_ERR_ALIGN: return "null or misaligned pointer (16-byte alignment required)";
+    case B200AWQ_ERR_ALIGN: return "null or misaligned pointer (16-byte alignment required), or a residual overlapping y";
     case B200AWQ_ERR_DTYPE: return "unsupported dtype (fp16 / bf16 only; gelu_quant: fp16 only)";
     case B200AWQ_ERR_BATCH: return "unsupported batch size for gemv kernel (1..7)";
     case B200AWQ_ERR_WORKSPACE: return "workspace too small";

@@ -291,8 +291,11 @@ void check_dtype(const torch::Tensor& t, at::ScalarType want, const char* fn, co
   TORCH_CHECK(t.scalar_type() == want, fn, ": ", what, " must be ", want, ", got ", t.scalar_type());
 }
 
+// layer_scale / residual: w8a8_linear_forward_cuda's operands (b200awq_w8a8_linear); without either this is the
+// reference's GEMM call (b200awq_w8a8_gemm).
 void w8a8_gemm(const torch::Tensor& in, const torch::Tensor& kernel, const torch::Tensor& wscales, const torch::Tensor& ascales,
-               torch::Tensor& out, const torch::Tensor* bias, const char* fn) {
+               torch::Tensor& out, const torch::Tensor* bias, const char* fn, const torch::Tensor* layer_scale = nullptr,
+               const torch::Tensor* residual = nullptr) {
   std::initializer_list<const torch::Tensor*> all = {&in, &kernel, &wscales, &ascales, &out};
   check_cuda_contig(all, fn);
   if (bias) check_cuda_contig({bias}, fn);
@@ -310,10 +313,29 @@ void w8a8_gemm(const torch::Tensor& in, const torch::Tensor& kernel, const torch
   TORCH_CHECK(kernel.size(0) == n && kernel.size(1) == k, fn, ": kernel must be [N, K] = [", n, ", ", k, "]");
   TORCH_CHECK(wscales.numel() >= n && ascales.numel() >= m, fn, ": wscales needs N, ascales M elements");
   if (bias) TORCH_CHECK(bias->numel() >= n, fn, ": bias needs N elements");
+  for (const torch::Tensor* t : {layer_scale, residual}) {
+    if (!t) continue;
+    check_cuda_contig({t}, fn);
+    TORCH_CHECK(t->device() == out.device(), fn, ": layer_scale / residual must be on out_feats' device");
+    check_dtype(*t, at::ScalarType::Half, fn, t == layer_scale ? "layer_scale" : "residual");
+  }
+  if (layer_scale) TORCH_CHECK(layer_scale->dim() == 1 && layer_scale->size(0) == n, fn, ": layer_scale must be [", n, "]");
+  if (residual) {
+    TORCH_CHECK(residual->sizes() == out.sizes(), fn, ": residual must have out_feats' shape ", out.sizes());
+    const uintptr_t r = reinterpret_cast<uintptr_t>(residual->data_ptr()), o = reinterpret_cast<uintptr_t>(out.data_ptr());
+    const uintptr_t bytes = (uintptr_t)out.numel() * 2u;
+    TORCH_CHECK(bytes == 0 || r >= o + bytes || o >= r + bytes, fn, ": residual must not share memory with out_feats");
+  }
   if (m == 0 || n == 0) return;
   const c10::cuda::CUDAGuard guard(in.device());
-  raise(b200awq_w8a8_gemm(in.data_ptr(), kernel.data_ptr(), wscales.data_ptr(), ascales.data_ptr(), bias ? bias->data_ptr() : nullptr,
-                          out.data_ptr(), (int)m, (int)n, (int)k, current_stream()));
+  void* bp = bias ? bias->data_ptr() : nullptr;
+  if (layer_scale || residual)
+    raise(b200awq_w8a8_linear(in.data_ptr(), kernel.data_ptr(), wscales.data_ptr(), ascales.data_ptr(), bp,
+                              layer_scale ? layer_scale->data_ptr() : nullptr, residual ? residual->data_ptr() : nullptr,
+                              out.data_ptr(), (int)m, (int)n, (int)k, current_stream()));
+  else
+    raise(b200awq_w8a8_gemm(in.data_ptr(), kernel.data_ptr(), wscales.data_ptr(), ascales.data_ptr(), bp, out.data_ptr(),
+                            (int)m, (int)n, (int)k, current_stream()));
 }
 
 int act_dtype(const torch::Tensor& t, const char* fn) {
@@ -333,6 +355,17 @@ void w8a8_gemm_forward_cuda(torch::Tensor _in_feats, torch::Tensor _kernel, torc
 void w8a8_gemm_fuse_bias_forward_cuda(torch::Tensor _in_feats, torch::Tensor _kernel, torch::Tensor _wscales,
                                       torch::Tensor _ascales, torch::Tensor _out_feats, torch::Tensor _bias) {
   w8a8_gemm(_in_feats, _kernel, _wscales, _ascales, _out_feats, &_bias, "w8a8_gemm_fuse_bias_forward_cuda");
+}
+
+// New entry (no counterpart in the reference's extension): w8a8_gemm[_fuse_bias]_forward_cuda followed by the vision
+// encoder layers' `out * ls` and `residual + out`, in the GEMM's launch and bit-identical to those PyTorch ops.  Writes
+// out_feats like the reference's W8A8 entries.  layer_scale [N] and residual (out_feats' shape) are fp16, contiguous and
+// on out_feats' device; residual must not share memory with out_feats.
+void w8a8_linear_forward_cuda(torch::Tensor _in_feats, torch::Tensor _kernel, torch::Tensor _wscales, torch::Tensor _ascales,
+                              torch::Tensor _out_feats, c10::optional<torch::Tensor> bias,
+                              c10::optional<torch::Tensor> layer_scale, c10::optional<torch::Tensor> residual) {
+  w8a8_gemm(_in_feats, _kernel, _wscales, _ascales, _out_feats, bias.has_value() ? &*bias : nullptr, "w8a8_linear_forward_cuda",
+            layer_scale.has_value() ? &*layer_scale : nullptr, residual.has_value() ? &*residual : nullptr);
 }
 
 // reference: w8a8/quantization.cu:97-112 (out int8 like input, scale fp16 [tokens])
@@ -660,6 +693,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mlp_front_forward_cuda", &mlp_front_forward_cuda, "silu(x Wgate^T) * (x Wup^T) for W4A16 weights, one call");
   m.def("w8a8_gemm_forward_cuda", &w8a8_gemm_forward_cuda, "our w8a8 gemm kernel");
   m.def("w8a8_gemm_fuse_bias_forward_cuda", &w8a8_gemm_fuse_bias_forward_cuda, "our w8a8 gemm fused bias kernel");
+  m.def("w8a8_linear_forward_cuda", &w8a8_linear_forward_cuda,
+        "W8A8 linear with the layer scale and residual in the same launch, into out_feats", py::arg("in_feats"),
+        py::arg("kernel"), py::arg("wscales"), py::arg("ascales"), py::arg("out_feats"), py::arg("bias") = py::none(),
+        py::arg("layer_scale") = py::none(), py::arg("residual") = py::none());
   m.def("invoke_quant", &invoke_quant, "fp16->int8 quantization");
   m.def("rms_norm_general", &rms_norm_general, py::arg("out"), py::arg("input"), py::arg("weight"), py::arg("bias"),
         py::arg("scaling"), py::arg("epsilon"), py::arg("use_per_token_quant") = true,

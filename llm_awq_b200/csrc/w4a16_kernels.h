@@ -189,9 +189,12 @@ int launch_flat(const void* x, const void* qw, const void* sc, const void* sz, v
 int launch_rmsnorm(const void* x, const void* gamma, void* y, float eps, int m, int n, int dtype, bool pdl, cudaStream_t stream);
 
 // W8A8 GEMM, int8 x [M, K] and w [N, K], fp16 y [M, N] with the reference's epilogue; bias may be null
-// (w8a8_wgmma.cu).  M >= 1, N % 8 == 0, K % 16 == 0.
+// (w8a8_wgmma.cu).  M >= 1, N % 8 == 0, K % 16 == 0.  With a layer scale [N] or a residual [M, N] (fp16, 16-byte
+// aligned, either may be null) the epilogue kernel multiplies the stored values by the layer scale and adds the
+// residual (b200awq_w8a8_linear); with both null this launches the plain kernel.
 int launch_w8a8_gemm(const void* x, const void* w, const void* wscales, const void* ascales, const void* bias, void* y,
-                     int M, int N, int K, bool pdl, cudaStream_t stream);
+                     int M, int N, int K, bool pdl, cudaStream_t stream, const void* layer_scale = nullptr,
+                     const void* residual = nullptr);
 
 // W8A8 row kernels, one CTA per row, rows of at most w8a8_row_limit() elements (w8a8_rowops.cu)
 int w8a8_row_limit();

@@ -7,7 +7,8 @@
 //   y[m, n] = rn_f16(f32(acc) * (ws[n] * as[m]))                  no bias   (w8a8_gemm_cuda.cu:893-899)
 //   y[m, n] = rn_f16(fma(as[m], f32(acc) * ws[n], bias[n]))        bias      (w8a8_gemm_cuda.cu:573-577)
 // with acc = sum_k x[m, k] w[n, k] exact in int32, every product / FMA flushing denormals like the reference's
-// fast-math build.
+// fast-math build.  Behind b200awq_w8a8_linear the store loop also applies the vision encoder layers' layer scale and
+// residual to the rounded y (w8a8_store_epilogue), in instantiations of their own.
 //
 // Tile: 128 tokens x 128 output channels, 128 k per pipeline stage (one 128-byte swizzle row per token / channel).
 //   * x [M, K] int8 and w [N, K] int8, both K-major, arrive by TMA; rows past M / N and k past K are zero-filled, so
@@ -59,11 +60,68 @@ __device__ __forceinline__ void wgmma_s8_n128(int (&d)[64], uint64_t adesc, uint
 
 __device__ __forceinline__ float ldg_h(const __half* p) { return __half2float(__ldg(p)); }
 
-template <bool kBias>
+// The layer scale and residual of b200awq_w8a8_linear on the 8 consecutive fp16 values v of one 16-byte store (the
+// tile's rn_f16 outputs), given the matching 16 B of the layer scale (l, if has_ls) and of the residual (r, if has_res):
+//   v = rn_f16(f32(v) * f32(l)), then v = rn_f16(f32(r) + f32(v))
+// one fp32 operation each, rounded once: PyTorch's fp16 `out * ls` and `residual + out` (products and sums of fp16
+// values are exact in fp32 and never subnormal there, so no flush can apply).
+__device__ __forceinline__ uint4 w8a8_epilogue_x8(uint4 v, bool has_ls, uint4 l, bool has_res, uint4 r) {
+  uint32_t vw[4] = {v.x, v.y, v.z, v.w};
+  const uint32_t lw[4] = {l.x, l.y, l.z, l.w}, rw[4] = {r.x, r.y, r.z, r.w};
+  auto f = [](uint32_t w, int h) { return __half2float(__ushort_as_half((unsigned short)(w >> (16 * h)))); };
+  auto bits = [](float x) { return (uint32_t)__half_as_ushort(__float2half_rn(x)); };
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    uint32_t o = 0;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      uint32_t e = (vw[q] >> (16 * h)) & 0xffffu;
+      if (has_ls) e = bits(__fmul_rn(f(e, 0), f(lw[q], h)));
+      if (has_res) e = bits(__fadd_rn(f(rw[q], h), f(e, 0)));
+      o |= e << (16 * h);
+    }
+    vw[q] = o;
+  }
+  return make_uint4(vw[0], vw[1], vw[2], vw[3]);
+}
+
+// b200awq_w8a8_linear's store loop over the staged fp16 tile (after the staging writes, which the barrier here
+// completes): thread e stores pieces e + 256 p of the tile, always the same 8 channels (one layer-scale load) and
+// kPieces rows 16 apart.  The residual rows are all loaded right after the barrier, before the first store; loaded
+// before it they would be live across the staging, which already fills the 96 registers two CTAs of 9 warps allow.
+// Rows at or past M and channels at or past N are neither read nor stored.
+__device__ __forceinline__ void w8a8_store_epilogue(const uint8_t* stage_out, __half* __restrict__ y, int M, int N, int m0,
+                                                    int n0, const __half* layer_scale, const __half* residual) {
+  constexpr int kPieces = kTM * (kTN / 8) / 256;
+  const int cc = threadIdx.x & 15, n = n0 + cc * 8, r0 = threadIdx.x >> 4;
+  const uint4 zero = make_uint4(0, 0, 0, 0);
+  const bool n_ok = n < N;
+  const uint4 lv = layer_scale && n_ok ? *reinterpret_cast<const uint4*>(layer_scale + n) : zero;
+  const __half* rp = residual + (size_t)(m0 + r0) * N + n;
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  uint4 rv[kPieces];
+#pragma unroll
+  for (int p = 0; p < kPieces; ++p)
+    rv[p] = residual && n_ok && m0 + r0 + 16 * p < M ? *reinterpret_cast<const uint4*>(rp + (size_t)p * 16 * N) : zero;
+  __half* yp = y + (size_t)(m0 + r0) * N + n;
+#pragma unroll
+  for (int p = 0; p < kPieces; ++p) {
+    if (n_ok && m0 + r0 + 16 * p < M) {
+      const uint4 v = *reinterpret_cast<const uint4*>(stage_out + (r0 + 16 * p) * kOutRow + cc * 16);
+      *reinterpret_cast<uint4*>(yp + (size_t)p * 16 * N) =
+          w8a8_epilogue_x8(v, layer_scale != nullptr, lv, residual != nullptr, rv[p]);
+    }
+  }
+}
+
+// Epi: empty for the GEMM entries' kernels, whose parameters are then exactly the reference epilogue's; or the
+// (layer_scale, residual) pointers of b200awq_w8a8_linear, applied by w8a8_store_epilogue in place of the plain store
+// loop.  The empty pack keeps the plain instantiations' code and (demangled) names what they were before the epilogue.
+template <bool kBias, typename... Epi>
 __global__ void __launch_bounds__(kThreads, 2)
 w8a8_wgmma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w,
                   const __half* __restrict__ wscales, const __half* __restrict__ ascales, const __half* __restrict__ bias,
-                  __half* __restrict__ y, int M, int N, int K) {
+                  __half* __restrict__ y, int M, int N, int K, Epi... epi) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);  // [kStages] TMA -> consumers
@@ -166,12 +224,16 @@ w8a8_wgmma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constan
       *reinterpret_cast<__half2*>(stage_out + (r_lo + 8 * h) * kOutRow + c * 2) = __floats2half2_rn(v0, v1);
     }
   }
-  asm volatile("bar.sync 1, 256;" ::: "memory");
-  for (int e = threadIdx.x; e < kTM * (kTN / 8); e += 256) {
-    const int r = e >> 4, cc = e & 15;
-    const int m = m0 + r, n = n0 + cc * 8;
-    if (m < M && n < N)
-      *reinterpret_cast<uint4*>(y + (size_t)m * N + n) = *reinterpret_cast<const uint4*>(stage_out + r * kOutRow + cc * 16);
+  if constexpr (sizeof...(Epi) != 0) {
+    w8a8_store_epilogue(stage_out, y, M, N, m0, n0, epi...);
+  } else {
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    for (int e = threadIdx.x; e < kTM * (kTN / 8); e += 256) {
+      const int r = e >> 4, cc = e & 15;
+      const int m = m0 + r, n = n0 + cc * 8;
+      if (m < M && n < N)
+        *reinterpret_cast<uint4*>(y + (size_t)m * N + n) = *reinterpret_cast<const uint4*>(stage_out + r * kOutRow + cc * 16);
+    }
   }
 }
 
@@ -189,19 +251,28 @@ int encode_kmajor_s8(EncodeTiledFn enc, CUtensorMap* tm, const void* p, int rows
 }  // namespace
 
 int launch_w8a8_gemm(const void* x, const void* w, const void* wscales, const void* ascales, const void* bias, void* y,
-                     int M, int N, int K, bool pdl, cudaStream_t stream) {
+                     int M, int N, int K, bool pdl, cudaStream_t stream, const void* layer_scale, const void* residual) {
   if (M < 1 || N < 8 || N % 8 || K < 16 || K % 16) return B200AWQ_ERR_SHAPE;
   EncodeTiledFn enc = get_encoder();
   if (!enc) return B200AWQ_ERR_DRIVER;
   CUtensorMap tm_x, tm_w;
   if (int e = encode_kmajor_s8(enc, &tm_x, x, M, K, kTM)) return e;
   if (int e = encode_kmajor_s8(enc, &tm_w, w, N, K, kTN)) return e;
+  const dim3 grid((unsigned)((N + kTN - 1) / kTN), (unsigned)((M + kTM - 1) / kTM));
+  if (layer_scale || residual) {  // b200awq_w8a8_linear's instantiations, only when either operand is given
+    using P = const __half*;
+    auto kern = bias ? w8a8_wgmma_kernel<true, P, P> : w8a8_wgmma_kernel<false, P, P>;
+    const cudaError_t ea = bias ? ensure_dyn_smem<w8a8_wgmma_kernel<true, P, P>>(kSmemBytes)
+                                : ensure_dyn_smem<w8a8_wgmma_kernel<false, P, P>>(kSmemBytes);
+    if (ea) return (int)ea;
+    return launch_kernel(kern, grid, dim3(kThreads), kSmemBytes, stream, pdl, 1, tm_x, tm_w, wscales, ascales, bias, y, M, N,
+                         K, static_cast<P>(layer_scale), static_cast<P>(residual));
+  }
   auto kern = bias ? w8a8_wgmma_kernel<true> : w8a8_wgmma_kernel<false>;
   const cudaError_t ea = bias ? ensure_dyn_smem<w8a8_wgmma_kernel<true>>(kSmemBytes)
                               : ensure_dyn_smem<w8a8_wgmma_kernel<false>>(kSmemBytes);
   if (ea) return (int)ea;
-  return launch_kernel(kern, dim3((unsigned)((N + kTN - 1) / kTN), (unsigned)((M + kTM - 1) / kTM)), dim3(kThreads),
-                       kSmemBytes, stream, pdl, 1, tm_x, tm_w, wscales, ascales, bias, y, M, N, K);
+  return launch_kernel(kern, grid, dim3(kThreads), kSmemBytes, stream, pdl, 1, tm_x, tm_w, wscales, ascales, bias, y, M, N, K);
 }
 
 }  // namespace b200awq

@@ -67,6 +67,8 @@ def lib() -> ctypes.CDLL:
         L.b200awq_rmsnorm.restype = ci
         L.b200awq_w8a8_gemm.argtypes = [vp, vp, vp, vp, vp, vp, ci, ci, ci, vp]
         L.b200awq_w8a8_gemm.restype = ci
+        L.b200awq_w8a8_linear.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, vp]
+        L.b200awq_w8a8_linear.restype = ci
         L.b200awq_quant_per_token.argtypes = [vp, vp, vp, ci, ci, ci, vp]
         L.b200awq_quant_per_token.restype = ci
         L.b200awq_layernorm_quant.argtypes = [vp, vp, vp, vp, vp, ci, ci, ctypes.c_float, ci, ci, vp]

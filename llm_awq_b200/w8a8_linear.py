@@ -46,10 +46,18 @@ class W8A8OF16LinearDynamicInputScale(torch.nn.Module):
             self.register_parameter("bias", None)
         self._fuse_bias = bool(bias)  # the reference picks its apply_weights at construction
 
-    def forward(self, input_, input_scale, output_buffer):
-        """input_ int8 [tokens, IC] codes, input_scale fp16 [tokens], output_buffer fp16 [tokens, OC] (written)."""
+    def forward(self, input_, input_scale, output_buffer, residual=None, layer_scale=None):
+        """input_ int8 [tokens, IC] codes, input_scale fp16 [tokens], output_buffer fp16 [tokens, OC] (written).
+
+        With `layer_scale` (fp16 [OC]) and / or `residual` (fp16, output_buffer's shape, not sharing its memory),
+        output_buffer receives `residual + out * layer_scale` in the GEMM's own launch, bit-identical to the encoder
+        layers' PyTorch ops on the plain output (InternViT's `residual + out * self.ls1`, SigLIP's `residual + out`)."""
         e = _get_engine()
-        if self._fuse_bias:
+        if residual is not None or layer_scale is not None:
+            e.w8a8_linear_forward_cuda(input_, self.weight, self.dequant_scale, input_scale, output_buffer,
+                                       bias=self.bias if self._fuse_bias else None, layer_scale=layer_scale,
+                                       residual=residual)
+        elif self._fuse_bias:
             e.w8a8_gemm_fuse_bias_forward_cuda(input_, self.weight, self.dequant_scale, input_scale, output_buffer, self.bias)
         else:
             e.w8a8_gemm_forward_cuda(input_, self.weight, self.dequant_scale, input_scale, output_buffer)
