@@ -6,10 +6,6 @@ The yardstick is the float64 definition in tests/prefill_attention_oracle.py ove
 tests/test_kv_cache_attention_cpu.py indexes the FT cache as oracle/layer_oracle.py does), with the tolerances of the
 other attention tests: 2e-3 (fp16) / 8e-3 (bf16) normwise per (batch row, head)."""
 import ctypes
-import json
-import os
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -17,6 +13,8 @@ import torch
 import llm_awq_b200 as P
 import attention_gqa_cases as C
 import prefill_attention_oracle as PO
+from guard_bands import Op, guarded_call
+from kernel_trace import trace
 from test_kv_cache_attention_cpu import FT, BTHD, ft_keys, ft_values, _tinychat_chunk_kv, _tinychat_store
 
 pytestmark = pytest.mark.gpu
@@ -173,45 +171,6 @@ def test_reads_only_its_slots_and_rows(layout, B, Sq, Sk, H, Hkv, D):
     _check(clean, q, k, v, True, D ** -0.5, dtype)
 
 
-GUARD = 4096
-
-
-def _guarded(call, ins, outs):
-    """Operands in buffers between GUARD-byte bands, run twice: inputs' bands NaN then zero, outputs and the workspace
-    (zeroed before the call) behind 0xA5 then 0x5A bands, outputs pre-filled with the same.  Every band and every input
-    byte must be unchanged, and both runs must write the same output bits."""
-    results = []
-    for run in (0, 1):
-        bufs, views = {}, {}
-        for name, t in list(ins.items()) + list(outs.items()):
-            nbytes = t.numel() * t.element_size()
-            buf = torch.empty(GUARD + nbytes + GUARD, dtype=torch.uint8, device=DEV)
-            if name in ins and run == 0:
-                buf.view(torch.int16).fill_(0x7E00)
-            elif name in ins:
-                buf.zero_()
-            else:
-                buf.fill_((0xA5, 0x5A)[run])
-            view = buf[GUARD:GUARD + nbytes].view(t.dtype).view(t.shape)
-            if name in ins:
-                view.copy_(t)
-            elif name == "ws":
-                view.zero_()
-            bufs[name], views[name] = (buf, buf.clone(), nbytes), view
-        assert call(views) == 0
-        torch.cuda.synchronize()
-        for name, (buf, before, nbytes) in bufs.items():
-            assert torch.equal(buf[:GUARD], before[:GUARD]), f"{name}: guard before written"
-            assert torch.equal(buf[GUARD + nbytes:], before[GUARD + nbytes:]), f"{name}: guard after written"
-            if name in ins:
-                assert torch.equal(buf, before), f"{name}: input written"
-        if "ws" in views:
-            assert int(torch.count_nonzero(views["ws"][:COUNTER_BYTES])) == 0, "counters not left zero"
-        results.append(views["out"].clone())
-    assert torch.equal(results[0].view(torch.int16), results[1].view(torch.int16)), "output differs between fills"
-    return results[0]
-
-
 @pytest.mark.parametrize("case", ["ft_sq17_g4", "ft_r130_d64", "bthd_sq129_g1", "ft_single_split", "bthd_sq65_g7"])
 def test_guard_bands(case):
     """Every operand, the workspace included, between 4 KiB guard bands: partial row tiles (R not a multiple of 8, of
@@ -226,53 +185,36 @@ def test_guard_bands(case):
     kc, vc = _caches(layout, B, L, Hkv, D, Sk, dtype, 9)
     need = P.lib().b200awq_kv_cache_attention_workspace_bytes(layout, B, Sq, Sk, H, Hkv, D)
     assert (need == 0) == (case == "ft_single_split")
-    outs = {"out": torch.empty_like(q)}
+    ops = {"q": Op("in", q), "k": Op("in", kc), "v": Op("in", vc), "out": Op("out", shape=q.shape, dtype=dtype)}
     if need:
-        outs["ws"] = torch.empty(need, dtype=torch.uint8, device=DEV)
+        ops["ws"] = Op("zeroed", shape=(need,), dtype=torch.uint8)
 
-    def call(vw):
-        ws = vw.get("ws", torch.empty(16, dtype=torch.uint8, device=DEV))
-        return _abi(vw["q"], vw["k"], vw["v"], vw["out"], layout, Sk, ws=ws, ws_bytes=need)
-    got = _guarded(call, {"q": q, "k": kc, "v": vc}, outs)
+    def call(v):
+        ws = v.get("ws", torch.empty(16, dtype=torch.uint8, device=DEV))
+        rc = _abi(v["q"], v["k"], v["v"], v["out"], layout, Sk, ws=ws, ws_bytes=need)
+        torch.cuda.synchronize()
+        assert not need or int(torch.count_nonzero(ws[:COUNTER_BYTES])) == 0, "counters not left zero"
+        return rc
+    got = guarded_call(call, ops)["out"]
     k, v = _logical(layout, kc, vc, B, Sk)
     _check(got, q, k, v, True, D ** -0.5, dtype)
 
 
-_PROFILE_ONE_KERNEL = """
-import json, sys
-sys.path[:0] = sys.argv[1:3]
-import torch
-import llm_awq_b200 as P
-eng = P.engine()
-res = {}
-B, L, H, Hkv, D = 1, 9000, 32, 8, 128
-kc = torch.randn(B, Hkv, D // 8, L, 8, device="cuda").half()
-vc = torch.randn(B, Hkv, L, D, device="cuda").half()
-kb = torch.randn(B, L, Hkv, D, device="cuda").half()
-vb = torch.randn(B, L, Hkv, D, device="cuda").half()
-for name, Sq, k, v in (("ft_sq17", 17, kc, vc), ("ft_sq300", 300, kc, vc), ("bthd_sq64", 64, kb, vb)):
-    qkv = torch.randn(B, Sq, H + 2 * Hkv, D, device="cuda").half()
-    q = qkv[:, :, :H]  # a strided view of the fused qkv output, read in place
-    eng.kv_cache_attention(q, k, v, 8500)
-    torch.cuda.synchronize()
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        eng.kv_cache_attention(q, k, v, 8500)
-        torch.cuda.synchronize()
-    res[name] = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-print(json.dumps(res))
-"""
+def traced_call(layout, Sq):
+    """kernel_trace builder: one call over a cache of 9000 slots, q a strided view of the fused qkv output, read in
+    place."""
+    B, L, H, Hkv, D = 1, 9000, 32, 8, 128
+    kc, vc = _caches(layout, B, L, Hkv, D, 8500, torch.float16, 1)
+    q = torch.randn(B, Sq, H + 2 * Hkv, D, device=DEV).half()[:, :, :H]
+    return lambda: P.engine().kv_cache_attention(q, kc, vc, 8500)
 
 
 def test_one_kernel_per_call():
-    """In a process of its own: each call over a cache, q a view of the fused qkv output, runs exactly one kernel (the
-    split-key kernel; the combine is inside it) and no copy, fill or elementwise kernel."""
-    tests = os.path.dirname(os.path.abspath(__file__))
-    r = subprocess.run([sys.executable, "-s", "-c", _PROFILE_ONE_KERNEL, os.path.dirname(tests), tests], capture_output=True,
-                       text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-3000:]
-    res = json.loads(r.stdout.strip().splitlines()[-1])
-    for name, kernels in res.items():
-        assert len(kernels) == 1 and "splitkv_attention_kernel" in kernels[0], (name, kernels)
+    """Each call over a cache, q a view of the fused qkv output, runs exactly one kernel (the split-key kernel; the
+    combine is inside it) and no copy, fill or elementwise kernel."""
+    cases = {"ft_sq17": (FT, 17), "ft_sq300": (FT, 300), "bthd_sq64": (BTHD, 64)}
+    for name, rec in zip(cases, trace("test_kv_cache_attention_gpu:traced_call", cases.values(), per_process=8)):
+        assert len(rec.names) == 1 and "splitkv_attention_kernel" in rec.names[0], (name, rec.names)
 
 
 # ------------------------------------------------------------------------------------------------ agreement

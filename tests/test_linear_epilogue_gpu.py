@@ -4,22 +4,18 @@ awq_inference_engine.w4a16_linear_forward_cuda, WQLinear.forward(x, residual)).
 The contract is bit-identity with what callers do today: the existing engine call (gemv_forward_cuda_new below 8
 tokens, gemm_forward_cuda_new from 8, the reference's dispatch rule) followed by PyTorch's `out + bias` and then
 `residual + out`.  Every comparison here is torch.equal.  The route each case takes is pinned by kernel name with the
-profiler, so that every kernel's epilogue (decode single-CTA and k-split cluster, ring, stream, the wgmma kernel's
-skinny launch and its tile launch with and without the split-k reduction) is covered by name.  Every profiler session
-runs in a process of its own (`profiled_kernels`), so that it cannot disturb the profiler tests that follow."""
+profiler (tests/kernel_trace.py), so that every kernel's epilogue (decode single-CTA and k-split cluster, ring, stream,
+the wgmma kernel's skinny launch and its tile launch with and without the split-k reduction) is covered by name."""
 import ctypes
-import json
 import os
-import re
-import subprocess
-import sys
 
 import pytest
 import torch
 
 import llm_awq_b200 as P
 from awq_testutil import gen_layer, gen_x
-from test_guard_bands_gpu import Op, guarded_call
+from guard_bands import Op, guarded_call
+from kernel_trace import short_names, trace
 from w4a16_plans import plan
 
 DEV = "cuda:0"
@@ -72,66 +68,26 @@ def fused(x, qw, s, z, bias=None, residual=None):
     return P.engine().w4a16_linear_forward_cuda(x, qw, s, z, 128, bias=bias, residual=residual)
 
 
-# Child process: for each case [m, n, k, dtype, entry, operands] the full names of the CUDA kernels of one call, after a
-# first call outside the profiled region (module load, descriptors).  entry "linear" is w4a16_linear_forward_cuda with
-# the given operands ("none", "bias", "residual", "both"), "engine" the gemv / gemm call of today.
-_PROFILE = """
-import json, sys
-sys.path[:0] = sys.argv[1:3]
-import torch
-import llm_awq_b200 as P
-from awq_testutil import gen_layer, gen_x
-eng = P.engine()
-out = []
-for m, n, k, dt, entry, op in json.loads(sys.argv[3]):
+def traced_call(m, n, k, dt, entry, op):
+    """kernel_trace builder: entry "linear" is w4a16_linear_forward_cuda with the given operands ("none", "bias",
+    "residual", "both"), "engine" the gemv / gemm call of today."""
     dtype = getattr(torch, dt)
+    eng = P.engine()
     qw, s, z = gen_layer(n, k, dtype, seed=n + k, device="cuda")
     x = gen_x(m, k, dtype, seed=m).cuda()
     bias = torch.randn(n, device="cuda").to(dtype) if op in ("bias", "both") else None
     res = torch.randn(m, n, device="cuda").to(dtype) if op in ("residual", "both") else None
     if entry == "linear":
-        call = lambda: eng.w4a16_linear_forward_cuda(x, qw, s, z, 128, bias=bias, residual=res)
-    elif m < 8:
-        call = lambda: eng.gemv_forward_cuda_new(x, qw, s, z, m, n, k, 128)
-    else:
-        call = lambda: eng.gemm_forward_cuda_new(x, qw, s, z)
-    call()
-    torch.cuda.synchronize()
-    for attempt in range(3):  # a session that recorded no kernel at all lost its activity records: profile again
-        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-            call()
-            torch.cuda.synchronize()
-        names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-        if names:
-            break
-    out.append(names)
-print(json.dumps(out))
-"""
+        return lambda: eng.w4a16_linear_forward_cuda(x, qw, s, z, 128, bias=bias, residual=res)
+    if m < 8:
+        return lambda: eng.gemv_forward_cuda_new(x, qw, s, z, m, n, k, 128)
+    return lambda: eng.gemm_forward_cuda_new(x, qw, s, z)
 
 
-def profiled_kernels(cases, env=None, per_process=8):
-    """Kernel names per case (see _PROFILE), profiled in processes of their own, a few profiler sessions each."""
-    tests = os.path.dirname(os.path.abspath(__file__))
+def profiled_kernels(cases, env=None):
+    """The names of the GPU work of one call per case (see traced_call), eight cases per profiling process."""
     cases = [[m, n, k, "float16" if dt == F16 else "bfloat16", entry, op] for m, n, k, dt, entry, op in cases]
-    out = []
-    for i in range(0, len(cases), per_process):
-        r = subprocess.run([sys.executable, "-s", "-c", _PROFILE, os.path.dirname(tests), tests,
-                            json.dumps(cases[i:i + per_process])],
-                           capture_output=True, text=True, timeout=900, env=dict(os.environ, **(env or {})))
-        assert r.returncode == 0, r.stderr[-3000:]
-        out += json.loads(r.stdout.strip().splitlines()[-1])
-    return out
-
-
-def short_names(names):
-    """The W4A16 kernels among `names` as `w4a16_<name>_kernel`, or `w4a16_wgmma_kernel<TN>` (TN is the wgmma kernel's
-    last template argument)."""
-    found = set()
-    for name in names:
-        mt = re.search(r"w4a16_(\w+?)_kernel(<[^>]*?(\d+)>)?", name)
-        if mt:
-            found.add(f"w4a16_wgmma_kernel<{mt.group(3)}>" if mt.group(1) == "wgmma" else f"w4a16_{mt.group(1)}_kernel")
-    return found
+    return [r.names for r in trace("test_linear_epilogue_gpu:traced_call", cases, per_process=8, env=env)]
 
 
 def check_equal(got, want, what):

@@ -1,9 +1,9 @@
 """The MLP front half (b200awq_w4a16_mlp_front: silu(x Wgate~^T) * (x Wup~^T)) at every plan it reaches on this device,
 at the partition edges its SM count puts in the shapes (w4a16_plans.mlp_front_cases).
 
-* The profiler pins each case's launches: the kernels in stream order, their grids and their shared memory equal what
-  w4a16_plans.mlp_front_plan() derives from the shape and the SM count.  The fused one-token kernel is told apart from
-  the plain decode kernel by its template arguments, w4a16_decode_kernel<true, false>.
+* The profiler pins each case's launches (tests/kernel_trace.py): the kernels in stream order, their grids and their
+  shared memory equal what w4a16_plans.mlp_front_plan() derives from the shape and the SM count.  The fused one-token
+  kernel is told apart from the plain decode kernel by its template arguments, w4a16_decode_kernel<true, false>.
 * Fused cases (one fp16 token): the kernel sums each product in the plain decode kernel's order and rounds like
   silu_mul_kernel, so y equals b200awq_w4a16_gemv(gate) | b200awq_w4a16_gemv(up) -> b200awq_silu_and_mul bit for bit
   (the mirror confirms that the plain plan has the same split and partition), on a probe token and on a randn token
@@ -24,9 +24,9 @@ import torch
 
 import llm_awq_b200 as P
 from awq_testutil import gen_layer
-from test_linear_epilogue_gpu import short_names
-from test_token_isolation_gpu import bound_violations, gamma, oracle_terms, probe_tokens
-from test_w4a16_plans_gpu import call, profiled_launches
+from kernel_trace import short_names, trace
+from oracle import w4a16_oracle as O
+from test_token_isolation_gpu import bound_violations, gamma, oracle_terms, probe_tokens, run
 from w4a16_plans import edge_channels, edge_tokens, mlp_front_cases, mlp_front_plan, plan
 
 pytestmark = pytest.mark.gpu
@@ -115,16 +115,30 @@ def launch_name(name):
     return found.pop() if found else name
 
 
+def traced_call(i):
+    """kernel_trace builder: b200awq_w4a16_mlp_front of CASES[i] on zero weights, with a workspace."""
+    c = CASES[i]
+    T = DTYPE[c.dtype]
+    x, y = torch.zeros(c.m, c.k, dtype=T, device=DEV), torch.empty(c.m, c.n, dtype=T, device=DEV)
+    gate, up = ((torch.zeros(c.n // 4, c.k, dtype=torch.int16, device=DEV),
+                 *(torch.zeros(O.scale_rows(c.k), c.n, dtype=T, device=DEV) for _ in range(2))) for _ in range(2))
+    nb = P.lib().b200awq_w4a16_mlp_front_workspace_bytes(c.m, c.n, c.k)
+    ws = torch.empty(nb, dtype=torch.uint8, device=DEV)
+    st = _st()
+    return lambda: P.lib().b200awq_w4a16_mlp_front(_p(x), *map(_p, gate), *map(_p, up), _p(y), c.m, c.n, c.k, 128,
+                                                   int(c.dtype == "bf16"), _p(ws), nb, st)
+
+
 def test_launches_pinned_by_profiler():
     name = torch.cuda.get_device_name(0)
-    launches = profiled_launches(CASES)
+    records = trace("test_mlp_front_plans_gpu:traced_call", [[i] for i in range(len(CASES))], per_process=64)
     rows, wrong = [], []
-    for c, got in zip(CASES, launches):
+    for c, rec in zip(CASES, records):
         ps = mlp_front_plan(c.m, c.n, c.k, c.dtype, SMS)
         # the trace gives static + dynamic shared memory: the stream kernel's 8 bytes of static exchange epochs take
         # one 128-byte unit, the other kernels have none
         want = [(p.kernel, [p.grid, 1, 1], p.smem + (128 if p.route == "stream" else 0)) for p in ps]
-        have = [(launch_name(n), g, sm) for n, g, sm in got]
+        have = [(launch_name(e.name), e.grid, e.smem) for e in rec.events]
         rows.append(f"| {c.id} | {', '.join(h[0] for h in have)} | {[h[1][0] for h in have]} | {[h[2] for h in have]} | "
                     f"{[w[2] for w in want]} |")
         if have != want:
@@ -145,7 +159,7 @@ def test_fused_equals_gemv_gemv_silu_and_mul(case):
     x, xd = tokens(c)
     rc, y, _ = mlp_front(xd, gate, up, workspace=False)   # the fused kernel needs no workspace
     assert rc == 0, P.lib().b200awq_strerror(rc)
-    g, u = call("gemv", xd, *gate), call("gemv", xd, *up)
+    g, u = run("gemv", xd, *gate), run("gemv", xd, *up)
     assert_bit_identical(y, silu_and_mul(g, u), f"{c.id}: fused against gemv | gemv -> silu_and_mul")
     assert_within_bound(g, x, gate, pp, f"{c.id} gate")
     assert_within_bound(u, x, up, pp, f"{c.id} up")
@@ -154,7 +168,7 @@ def test_fused_equals_gemv_gemv_silu_and_mul(case):
     xr = torch.randn(1, c.k, generator=torch.Generator().manual_seed(c.k)).to(torch.float16).to(DEV)
     rc, y, _ = mlp_front(xr, gate, up, workspace=False)
     assert rc == 0, P.lib().b200awq_strerror(rc)
-    g, u = call("gemv", xr, *gate), call("gemv", xr, *up)
+    g, u = run("gemv", xr, *gate), run("gemv", xr, *up)
     assert torch.isfinite(g).all() and torch.isfinite(u).all()
     assert_bit_identical(y, silu_and_mul(g, u), f"{c.id}: fused against gemv | gemv -> silu_and_mul on a randn token")
 
@@ -177,8 +191,8 @@ def test_composed_products_within_bound_and_silu_and_mul_exact(case):
     same = [e for e in ("gemv", "gemm") if (e == "gemm" or c.m <= 7) and (e == "gemv" or c.n % 128 == 0)
             and plan(c.m, c.n, c.k, c.dtype, e, SMS) == p]
     for e in same:
-        assert_bit_identical(g, call(e, xd, *gate), f"{c.id}: gate product against the {e} entry (same plan)")
-        assert_bit_identical(u, call(e, xd, *up), f"{c.id}: up product against the {e} entry (same plan)")
+        assert_bit_identical(g, run(e, xd, *gate), f"{c.id}: gate product against the {e} entry (same plan)")
+        assert_bit_identical(u, run(e, xd, *up), f"{c.id}: up product against the {e} entry (same plan)")
 
 
 # ------------------------------------------------------------------------------------------------ plugin and module

@@ -6,10 +6,7 @@ Tolerances are those of the decode-attention tests: 2e-3 (fp16) / 8e-3 (bf16) no
 cases check every row of sampled heads, the first and the last among them."""
 import ctypes
 import importlib.util
-import json
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -19,7 +16,8 @@ import llm_awq_b200 as P
 import attention_gqa_cases as C
 import prefill_attention_oracle as PO
 from awq_testutil import np64
-from test_guard_bands_gpu import Op, guarded_call
+from guard_bands import Op, guarded_call
+from kernel_trace import trace
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -104,31 +102,16 @@ def test_siglip_views(S, B, dtype):
     _check(out, q, k, v, False, 72 ** -0.5, dtype, heads=list(range(16)) if B == 1 else None)
 
 
-_PROFILE_SIGLIP = """
-import json, sys
-sys.path[:0] = sys.argv[1:3]
-import torch
-import llm_awq_b200 as P
-from test_prefill_attention_gpu import _siglip_qkv
-eng = P.engine()
-q, k, v = _siglip_qkv(2, 729, 16, 72, torch.float16, 5)
-eng.flash_attn_func(q, k, v)
-torch.cuda.synchronize()
-with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-    eng.flash_attn_func(q, k, v)
-    torch.cuda.synchronize()
-print(json.dumps(sorted({e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA})))
-"""
+def traced_call():
+    """kernel_trace builder: flash_attn_func on SigLIP's views of a fused qkv buffer."""
+    q, k, v = _siglip_qkv(2, 729, 16, 72, torch.float16, 5)
+    return lambda: P.engine().flash_attn_func(q, k, v)
 
 
 def test_siglip_views_are_not_copied():
-    """The profiler (in a process of its own, so that its session cannot disturb later profiler tests) sees the
-    attention kernel and no copy kernel."""
-    tests = os.path.dirname(os.path.abspath(__file__))
-    r = subprocess.run([sys.executable, "-s", "-c", _PROFILE_SIGLIP, os.path.dirname(tests), tests], capture_output=True,
-                       text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-3000:]
-    names = json.loads(r.stdout.strip().splitlines()[-1])
+    """The profiler sees the attention kernel and no copy kernel."""
+    (rec,) = trace("test_prefill_attention_gpu:traced_call", [[]], per_process=8)
+    names = rec.names
     assert any("prefill_attention_kernel" in n for n in names), names
     assert not any(("copy" in n.lower() or "elementwise" in n.lower()) for n in names), names
 

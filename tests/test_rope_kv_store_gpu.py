@@ -6,17 +6,14 @@ The yardstick is the composed route this entry replaces: this build's fused_rope
 tests/test_kv_cache_attention_cpu.py for the FT caches, slice assignment for the BTHD caches).  The new entry must
 match it bit for bit; caches and outputs are compared as 16-bit patterns, so poisoned NaNs compare too."""
 import ctypes
-import json
-import os
-import subprocess
-import sys
 
 import pytest
 import torch
 
 import llm_awq_b200 as P
 from awq_testutil import gen_layer
-from test_guard_bands_gpu import Op, guarded_call, _code, _p, _st
+from guard_bands import Op, guarded_call, _code, _p, _st
+from kernel_trace import trace
 from test_kv_cache_attention_cpu import FT, BTHD, _tinychat_chunk_kv, _tinychat_store
 from test_rope_kv_store_cpu import cache_shapes, poisoned
 
@@ -225,46 +222,20 @@ def test_launch_count():
         assert q.shape == (B, S, H, D)
 
 
-_PROFILE = """
-import json, sys
-sys.path[:0] = sys.argv[1:3]
-import torch
-import llm_awq_b200 as P
-eng = P.engine()
-res = {}
-H, Hkv, D, L = 32, 8, 128, 2048
-for name, B, S, dims in (("ft_s17", 1, 17, 5), ("ft_s512_b2", 2, 512, 5), ("bthd_s1", 1, 1, 4), ("bthd_s64", 2, 64, 4)):
-    if dims == 5:
-        kc = torch.zeros(B, Hkv, D // 8, L, 8, device="cuda").half()
-        vc = torch.zeros(B, Hkv, L, D, device="cuda").half()
-    else:
-        kc = torch.zeros(B, L, Hkv, D, device="cuda").half()
-        vc = torch.zeros(B, L, Hkv, D, device="cuda").half()
-    qkv = torch.randn(B, S, H + 2 * Hkv, D, device="cuda").half()
-    freqs = torch.rand(S, 1, 1, D, device="cuda")
-    eng.rope_kv_store(qkv, freqs, kc, vc, 100)
-    torch.cuda.synchronize()
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        eng.rope_kv_store(qkv, freqs, kc, vc, 100)
-        torch.cuda.synchronize()
-    res[name] = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-print(json.dumps(res))
-"""
+def traced_call(B, S, layout):
+    """kernel_trace builder: one rope_kv_store call of a chunk, with tinychat's [S, 1, 1, D] freqs slice."""
+    H, Hkv, D, L = 32, 8, 128, 2048
+    kc, vc = _caches(layout, B, Hkv, D, L, torch.float16)
+    qkv = torch.randn(B, S, H + 2 * Hkv, D, device=DEV).half()
+    freqs = torch.rand(S, 1, 1, D, device=DEV)
+    return lambda: P.engine().rope_kv_store(qkv, freqs, kc, vc, 100)
 
 
 def test_one_kernel_per_call():
-    """In a process of its own: each call (tinychat's [S, 1, 1, D] freqs slice included) runs exactly one kernel, the
-    rope_kv_store kernel, and no copy or fill."""
-    tests = os.path.dirname(os.path.abspath(__file__))
-    for attempt in range(3):  # a profiler session on a shared GPU occasionally records no CUDA activity at all
-        r = subprocess.run([sys.executable, "-s", "-c", _PROFILE, os.path.dirname(tests), tests], capture_output=True,
-                           text=True, timeout=600)
-        assert r.returncode == 0, r.stderr[-3000:]
-        res = json.loads(r.stdout.strip().splitlines()[-1])
-        if all(res.values()):
-            break
-    for name, kernels in res.items():
-        assert len(kernels) == 1 and "rope_kv_store_kernel" in kernels[0], (name, kernels)
+    """Each call runs exactly one kernel, the rope_kv_store kernel, and no copy or fill."""
+    cases = {"ft_s17": (1, 17, FT), "ft_s512_b2": (2, 512, FT), "bthd_s1": (1, 1, BTHD), "bthd_s64": (2, 64, BTHD)}
+    for name, rec in zip(cases, trace("test_rope_kv_store_gpu:traced_call", cases.values(), per_process=8)):
+        assert len(rec.names) == 1 and "rope_kv_store_kernel" in rec.names[0], (name, rec.names)
 
 
 # ------------------------------------------------------------------------------------------------ tinychat, multi-round

@@ -5,10 +5,6 @@ kernel.
 The yardstick is the float64 definition in tests/prefill_attention_oracle.py, with the tolerances of the other attention
 tests: 2e-3 (fp16) / 8e-3 (bf16) normwise per (batch row, head)."""
 import ctypes
-import json
-import os
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -16,7 +12,9 @@ import torch
 import llm_awq_b200 as P
 import attention_gqa_cases as C
 import prefill_attention_oracle as PO
-from test_guard_bands_gpu import Op, guarded_call
+from guard_bands import Op, guarded_call
+from kernel_trace import trace
+from test_prefill_attention_gpu import _siglip_qkv
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -328,47 +326,29 @@ def test_shared_workspace_grows_without_freeing_a_captured_buffer():
 
 
 # ------------------------------------------------------------------------------------------------ routes
-_PROFILE_ROUTES = """
-import json, sys
-sys.path[:0] = sys.argv[1:3]
-import torch
-import llm_awq_b200 as P
-from test_prefill_attention_gpu import _siglip_qkv
-eng = P.engine()
-def rnd(*s):
-    return torch.randn(*s, device="cuda").half()
-B, L, Hkv, D = 1, 9000, 8, 128
-kc, vc = rnd(B, L, Hkv, D), rnd(B, L, Hkv, D)
-calls = {
-    "decode_view": lambda: eng.flash_attn_func(rnd(B, 1, 32, D), kc[:, :8200], vc[:, :8200], causal=True),
-    "sq17_g4": lambda: eng.flash_attn_func(rnd(1, 17, 32, D), kc[:, :4000], vc[:, :4000], causal=True),
-    "chunk512": lambda: eng.flash_attn_func(rnd(1, 512, 32, D), kc[:, :2048], vc[:, :2048], causal=True),
-    "siglip": lambda: eng.flash_attn_func(*_siglip_qkv(2, 729, 16, 72, torch.float16, 5)),
-    "internvit": lambda: eng.flash_attn_varlen_qkvpacked_func(
-        rnd(2 * 1025, 3, 16, 64), torch.tensor([0, 1025, 2050], dtype=torch.int32, device="cuda"), 1025),
-}
-res = {}
-for name, fn in calls.items():
-    fn()
-    torch.cuda.synchronize()
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    res[name] = sorted({e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA})
-print(json.dumps(res))
-"""
+def traced_call(name):
+    """kernel_trace builder: the calls of test_routes and test_decode_over_a_cache_view_is_not_copied, their inputs
+    made before the call."""
+    eng = P.engine()
+    rnd = lambda *s: torch.randn(*s, device=DEV).half()  # noqa: E731
+    if name == "siglip":
+        qkv = _siglip_qkv(2, 729, 16, 72, torch.float16, 5)
+        return lambda: eng.flash_attn_func(*qkv)
+    if name == "internvit":
+        qkv, cu = rnd(2 * 1025, 3, 16, 64), torch.tensor([0, 1025, 2050], dtype=torch.int32, device=DEV)
+        return lambda: eng.flash_attn_varlen_qkvpacked_func(qkv, cu, 1025)
+    B, Sq, Sk = {"decode_view": (1, 1, 8200), "sq17_g4": (1, 17, 4000), "chunk512": (1, 512, 2048),
+                 "decode_b2": (2, 1, 8200)}[name]
+    kc, vc, q = rnd(B, 9000, 8, 128), rnd(B, 9000, 8, 128), rnd(B, Sq, 32, 128)
+    return lambda: eng.flash_attn_func(q, kc[:, :Sk], vc[:, :Sk], causal=True)
 
 
 def test_routes():
-    """In a process of its own (its profiler session cannot disturb later tests): a single query over a cache view runs
-    the split-key kernel; Sq * G > 64, a 512-token chunk, SigLIP and InternViT run the prefill kernel.  (The calls build
-    their queries inside the profiled region; test_decode_over_a_cache_view_is_not_copied checks that nothing but the
-    kernel runs.)"""
-    tests = os.path.dirname(os.path.abspath(__file__))
-    r = subprocess.run([sys.executable, "-s", "-c", _PROFILE_ROUTES, os.path.dirname(tests), tests], capture_output=True,
-                       text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-3000:]
-    res = json.loads(r.stdout.strip().splitlines()[-1])
+    """A single query over a cache view runs the split-key kernel; Sq * G > 64, a 512-token chunk, SigLIP and InternViT
+    run the prefill kernel."""
+    cases = ["decode_view", "sq17_g4", "chunk512", "siglip", "internvit"]
+    res = {c: r.names for c, r in zip(cases, trace("test_splitkv_attention_gpu:traced_call", [[c] for c in cases],
+                                                   per_process=8))}
     assert any("splitkv_attention_kernel" in n for n in res["decode_view"]), res["decode_view"]
     assert not any("prefill_attention_kernel" in n for n in res["decode_view"]), res["decode_view"]
     for name in ("sq17_g4", "chunk512", "siglip", "internvit"):
@@ -376,32 +356,9 @@ def test_routes():
         assert not any("splitkv_attention_kernel" in n for n in res[name]), (name, res[name])
 
 
-_PROFILE_NO_COPY = """
-import json, sys
-sys.path[:0] = sys.argv[1:3]
-import torch
-import llm_awq_b200 as P
-eng = P.engine()
-B, L, H, Hkv, D = 2, 9000, 32, 8, 128
-kc = torch.randn(B, L, Hkv, D, device="cuda").half()
-vc = torch.randn(B, L, Hkv, D, device="cuda").half()
-q = torch.randn(B, 1, H, D, device="cuda").half()
-k, v = kc[:, :8200], vc[:, :8200]
-eng.flash_attn_func(q, k, v, causal=True)
-torch.cuda.synchronize()
-with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-    eng.flash_attn_func(q, k, v, causal=True)
-    torch.cuda.synchronize()
-print(json.dumps(sorted({e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA})))
-"""
-
-
 def test_decode_over_a_cache_view_is_not_copied():
-    tests = os.path.dirname(os.path.abspath(__file__))
-    r = subprocess.run([sys.executable, "-s", "-c", _PROFILE_NO_COPY, os.path.dirname(tests), tests], capture_output=True,
-                       text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-3000:]
-    names = json.loads(r.stdout.strip().splitlines()[-1])
+    (rec,) = trace("test_splitkv_attention_gpu:traced_call", [["decode_b2"]], per_process=8)
+    names = rec.names
     assert any("splitkv_attention_kernel" in n for n in names), names
     assert not any(("copy" in n.lower() or "elementwise" in n.lower() or "fill" in n.lower()) for n in names), names
 

@@ -24,11 +24,11 @@ oracle in float64 with w~ = rn_T(q s + z), A = |x| . |w~|^T, and
     (DESIGN.md 3.1).  Zero on every other route.
 Where the oracle's value rounded to T overflows, the output must be an infinity of the same sign.
 
-The profiler test pins the kernel each case runs, so a change of the dispatch cannot quietly move a case to another
-route.  The bound itself is tested on the CPU: the oracle rounded to T passes, and an output missing one group's
-contribution in a single element, or using the neighbouring channel's scale in a single element, fails."""
+The profiler test (tests/kernel_trace.py) pins the kernel each case runs, so a change of the dispatch cannot quietly
+move a case to another route.  The bound itself is tested on the CPU: the oracle rounded to T passes, and an output
+missing one group's contribution in a single element, or using the neighbouring channel's scale in a single element,
+fails."""
 import ctypes
-import re
 
 import numpy as np
 import pytest
@@ -36,6 +36,7 @@ import torch
 
 import llm_awq_b200 as P
 from awq_testutil import gen_layer
+from kernel_trace import short_names, trace
 from oracle import w4a16_oracle as O
 from w4a16_plans import plan
 
@@ -166,12 +167,13 @@ def bound_violations(y, Y, A, D, dtype, gam, digits):
 
 
 # ------------------------------------------------------------------------------------------------ calls
-def run(entry, x, qw, s, z, dtype):
+def run(entry, x, qw, s, z):
+    """y of b200awq_w4a16_gemv / _gemm, into a NaN-filled buffer."""
     M, K = x.shape
     N = s.shape[1]
-    y = torch.empty(M, N, dtype=dtype, device=DEV)
+    y = torch.full((M, N), float("nan"), dtype=x.dtype, device=DEV)
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    code = 0 if dtype == F16 else 1
+    code = 0 if x.dtype == F16 else 1
     L = P.lib()
     if entry == "gemv":
         rc = L.b200awq_w4a16_gemv(x.data_ptr(), qw.data_ptr(), s.data_ptr(), z.data_ptr(), y.data_ptr(), M, N, K, 128, code, st)
@@ -193,8 +195,8 @@ def test_probe_tokens_isolated_and_within_elementwise_bound(case):
     route, M, N, K, dtype, entry = case
     qw, s, z = layer(N, K, dtype)
     x_ext, x_ord, pr = batches(M, K, dtype, seed=M * 7 + K)
-    y_ext = run(entry, x_ext.to(DEV), qw, s, z, dtype)
-    y_ord = run(entry, x_ord.to(DEV), qw, s, z, dtype)
+    y_ext = run(entry, x_ext.to(DEV), qw, s, z)
+    y_ord = run(entry, x_ord.to(DEV), qw, s, z)
     torch.cuda.synchronize()
     for i in pr:
         assert torch.equal(y_ext[i].view(torch.int16), y_ord[i].view(torch.int16)), f"probe token {i} depends on its neighbours"
@@ -213,32 +215,22 @@ def expected_kernel(route, M, N, K, dtype, entry, sms):
     return p.kernel
 
 
-def kernels_run(fn):
-    """Names of the W4A16 kernels fn launches, as `w4a16_<name>_kernel` or `w4a16_wgmma_kernel<TN>`."""
-    for attempt in range(3):  # a session that recorded no kernel at all lost its activity records: profile again
-        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-            fn()
-            torch.cuda.synchronize()
-        found = set()
-        for ev in prof.events():
-            m = re.search(r"w4a16_(\w+?)_kernel(<[^>]*?(\d+)>)?", ev.name)
-            if m:
-                found.add(f"w4a16_wgmma_kernel<{m.group(3)}>" if m.group(1) == "wgmma" else f"w4a16_{m.group(1)}_kernel")
-        if found:
-            break
-    return found
+def traced_call(i):
+    """kernel_trace builder: CASES[i]'s entry on a randn batch."""
+    route, M, N, K, dtype, entry = CASES[i]
+    qw, s, z = layer(N, K, dtype)
+    x = torch.randn(M, K).to(dtype).to(DEV)
+    return lambda: run(entry, x, qw, s, z)
 
 
 @pytest.mark.gpu
 def test_routes_pinned_by_profiler():
     sms = torch.cuda.get_device_properties(0).multi_processor_count
+    records = trace("test_token_isolation_gpu:traced_call", [[i] for i in range(len(CASES))], per_process=64)
     rows, wrong = [], []
-    for case in CASES:
+    for case, rec in zip(CASES, records):
         route, M, N, K, dtype, entry = case
-        qw, s, z = layer(N, K, dtype)
-        x = torch.randn(M, K).to(dtype).to(DEV)
-        run(entry, x, qw, s, z, dtype)                 # first launch (module load, descriptors) outside the trace
-        got = kernels_run(lambda: run(entry, x, qw, s, z, dtype))
+        got = short_names(rec.names)
         want = expected_kernel(route, M, N, K, dtype, entry, sms)
         rows.append(f"| {route} | {M} | {N} | {K} | {TAG[dtype]} | {entry} | {', '.join(sorted(got))} |")
         if got != {want}:

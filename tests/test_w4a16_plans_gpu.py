@@ -1,8 +1,8 @@
 """Every W4A16 plan the dispatch reaches on this device, at the partition edges its SM count puts in the shapes
 (w4a16_plans.edge_cases), against the float64 oracle element by element.
 
-* The profiler pins each case's plan: the kernel's name, grid and shared memory in the exported trace equal what
-  w4a16_plans.plan() derives from the shape and the SM count (the shared memory pins the ring depths).
+* The profiler pins each case's plan: the kernel's name, grid and shared memory in its trace (tests/kernel_trace.py)
+  equal what w4a16_plans.plan() derives from the shape and the SM count (the shared memory pins the ring depths).
 * Each case's output is checked on the channels and tokens that carry the plan's edges (w4a16_plans.edge_channels,
   edge_tokens) with the elementwise bound of test_token_isolation_gpu.py, on AWQ-like probe tokens (outliers, a
   non-zero-mean group, subnormals).  The output buffer starts as NaN, so an element no CTA stores fails.
@@ -10,10 +10,6 @@
 * Every served projection (w4a16_plans.SERVED) at the token counts of the route boundaries, and at one token count
   where the tile launch splits k and its clusters walk several tiles, under the same bound."""
 import ctypes
-import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -21,8 +17,9 @@ import torch
 
 import llm_awq_b200 as P
 from awq_testutil import gen_layer
-from test_linear_epilogue_gpu import short_names
-from test_token_isolation_gpu import bound_violations, gamma, oracle_terms, probe_tokens
+from kernel_trace import short_names, trace
+from oracle import w4a16_oracle as O
+from test_token_isolation_gpu import bound_violations, gamma, oracle_terms, probe_tokens, run
 from w4a16_plans import edge_cases, edge_channels, edge_tokens, plan, served_shapes
 
 pytestmark = pytest.mark.gpu
@@ -34,23 +31,6 @@ CASES = edge_cases(SMS)
 BOUNDARY_MS = (1, 4, 5, 7, 8, 9, 16, 17)
 
 
-def call(entry, x, qw, s, z):
-    """y of b200awq_w4a16_gemv / _gemm, into a NaN-filled buffer."""
-    M, K = x.shape
-    N = s.shape[1]
-    y = torch.full((M, N), float("nan"), dtype=x.dtype, device=DEV)
-    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    code = 0 if x.dtype == torch.float16 else 1
-    L = P.lib()
-    if entry == "gemv":
-        rc = L.b200awq_w4a16_gemv(x.data_ptr(), qw.data_ptr(), s.data_ptr(), z.data_ptr(), y.data_ptr(), M, N, K, 128, code, st)
-    else:
-        rc = L.b200awq_w4a16_gemm(x.data_ptr(), qw.data_ptr(), s.data_ptr(), z.data_ptr(), y.data_ptr(), M, N, K, 128, code,
-                                  None, 0, st)
-    assert rc == 0, L.b200awq_strerror(rc)
-    return y
-
-
 def check_plan_output(m, n, k, dtype, entry, what, layer=None):
     """Run the shape on probe tokens; the edge channels and tokens of its plan within the elementwise bound; a second
     launch bit-identical where the plan splits k."""
@@ -59,9 +39,9 @@ def check_plan_output(m, n, k, dtype, entry, what, layer=None):
     qw, s, z = layer or gen_layer(n, k, T, seed=n + 3 * k, device=DEV)
     x = probe_tokens(m, k, seed=m * 7 + k).to(T)
     xd = x.to(DEV)
-    y = call(entry, xd, qw, s, z)
+    y = run(entry, xd, qw, s, z)
     if p.S > 1:
-        y2 = call(entry, xd, qw, s, z)
+        y2 = run(entry, xd, qw, s, z)
         assert torch.equal(y.view(torch.int16), y2.view(torch.int16)), f"{what}: split-k plan {p} is not deterministic"
     toks, cols = edge_tokens(p, m), edge_channels(p, n)
     Y, A, D = oracle_terms(x[toks], qw, s, z, T, cols=cols)
@@ -76,76 +56,27 @@ def check_plan_output(m, n, k, dtype, entry, what, layer=None):
 
 
 # ------------------------------------------------------------------------------------------------ plans pinned
-# Child process: for each case [m, n, k, dtype, entry], (name, grid, shared memory) of every kernel of one call in launch
-# order, read from the exported Chrome trace, after a first call outside the profiled region (module load, descriptors).
-# Entry "mlp_front" is b200awq_w4a16_mlp_front with both weight sets and a workspace.
-_PROFILE = """
-import ctypes, json, os, sys, tempfile
-sys.path[:0] = sys.argv[1:3]
-import torch
-import llm_awq_b200 as P
-from oracle import w4a16_oracle as O
-L = P.lib()
-out = []
-for m, n, k, dt, entry in json.loads(sys.argv[3]):
-    dtype = torch.float16 if dt == "f16" else torch.bfloat16
-    x = torch.zeros(m, k, dtype=dtype, device="cuda")
-    qw = torch.zeros(n // 4, k, dtype=torch.int16, device="cuda")
-    s = torch.zeros(O.scale_rows(k), n, dtype=dtype, device="cuda")
-    z = torch.zeros_like(s)
-    y = torch.empty(m, n, dtype=dtype, device="cuda")
+def traced_call(i):
+    """kernel_trace builder: CASES[i]'s entry on zero operands."""
+    c = CASES[i]
+    T = DTYPE[c.dtype]
+    x, y = torch.zeros(c.m, c.k, dtype=T, device=DEV), torch.empty(c.m, c.n, dtype=T, device=DEV)
+    qw = torch.zeros(c.n // 4, c.k, dtype=torch.int16, device=DEV)
+    s, z = (torch.zeros(O.scale_rows(c.k), c.n, dtype=T, device=DEV) for _ in range(2))
+    args = [t.data_ptr() for t in (x, qw, s, z, y)] + [c.m, c.n, c.k, 128, int(c.dtype == "bf16")]
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    code = 0 if dt == "f16" else 1
-    if entry == "mlp_front":
-        qw2, s2, z2 = torch.zeros_like(qw), torch.zeros_like(s), torch.zeros_like(z)
-        nb = L.b200awq_w4a16_mlp_front_workspace_bytes(m, n, k)
-        ws = torch.empty(nb, dtype=torch.uint8, device="cuda")
-        run = lambda: L.b200awq_w4a16_mlp_front(x.data_ptr(), qw.data_ptr(), s.data_ptr(), z.data_ptr(), qw2.data_ptr(), s2.data_ptr(), z2.data_ptr(), y.data_ptr(), m, n, k, 128, code, ws.data_ptr(), nb, st)
-    elif entry == "gemv":
-        run = lambda: L.b200awq_w4a16_gemv(x.data_ptr(), qw.data_ptr(), s.data_ptr(), z.data_ptr(), y.data_ptr(), m, n, k, 128, code, st)
-    else:
-        run = lambda: L.b200awq_w4a16_gemm(x.data_ptr(), qw.data_ptr(), s.data_ptr(), z.data_ptr(), y.data_ptr(), m, n, k, 128, code, None, 0, st)
-    assert run() == 0
-    torch.cuda.synchronize()
-    for attempt in range(3):  # a session that recorded no kernel at all lost its activity records: profile again
-        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-            assert run() == 0
-            torch.cuda.synchronize()
-        fd, path = tempfile.mkstemp(suffix=".json")
-        os.close(fd)
-        try:
-            prof.export_chrome_trace(path)
-            with open(path) as f:
-                events = json.load(f)["traceEvents"]
-        finally:
-            os.unlink(path)
-        kernels = [[e["name"], e.get("args", {}).get("grid"), e.get("args", {}).get("shared memory")]
-                   for e in sorted((e for e in events if e.get("cat") == "kernel"), key=lambda e: e.get("ts", 0))]
-        if kernels:
-            break
-    out.append(kernels)
-print(json.dumps(out))
-"""
-
-
-def profiled_launches(cases, per_process=64):
-    tests = os.path.dirname(os.path.abspath(__file__))
-    rows = [[c.m, c.n, c.k, c.dtype, c.entry] for c in cases]
-    out = []
-    for i in range(0, len(rows), per_process):
-        r = subprocess.run([sys.executable, "-s", "-c", _PROFILE, os.path.dirname(tests), tests,
-                            json.dumps(rows[i:i + per_process])], capture_output=True, text=True, timeout=900)
-        assert r.returncode == 0, r.stderr[-3000:]
-        out += json.loads(r.stdout.strip().splitlines()[-1])
-    return out
+    if c.entry == "gemv":
+        return lambda: P.lib().b200awq_w4a16_gemv(*args, st)
+    return lambda: P.lib().b200awq_w4a16_gemm(*args, None, 0, st)
 
 
 def test_plans_pinned_by_profiler():
     name = torch.cuda.get_device_name(0)
-    launches = profiled_launches(CASES)
+    records = trace("test_w4a16_plans_gpu:traced_call", [[i] for i in range(len(CASES))], per_process=64)
     rows, wrong = [], []
-    for c, got in zip(CASES, launches):
+    for c, rec in zip(CASES, records):
         p = plan(c.m, c.n, c.k, c.dtype, c.entry, SMS)
+        got = [(e.name, e.grid, e.smem) for e in rec.events]
         names = short_names(n for n, _, _ in got)
         grids = [g for _, g, _ in got]
         smem = [sm for _, _, sm in got]

@@ -3,21 +3,18 @@ awq_inference_engine.w8a8_linear_forward_cuda, W8A8OF16LinearDynamicInputScale.f
 
 The contract is bit-identity with what tinychat's encoder layers do today: the W8A8 GEMM entry
 (w8a8_gemm[_fuse_bias]_forward_cuda) followed by PyTorch's fp16 `out * ls` and then `residual + out`.  Every comparison
-here is torch.equal on the 16-bit patterns.  Profiler sessions run in processes of their own (`profiled_kernels`), so
-that they cannot disturb the profiler tests that follow."""
+here is torch.equal on the 16-bit patterns.  Kernel names come from the profiler (tests/kernel_trace.py)."""
 import ctypes
 import json
-import os
 import re
-import subprocess
-import sys
 
 import pytest
 import torch
 
 import llm_awq_b200 as P
 import w8a8_cases as W
-from test_guard_bands_gpu import Op, guarded_call
+from guard_bands import Op, guarded_call
+from kernel_trace import trace
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -139,56 +136,21 @@ def test_extreme_operands():
 
 
 # ------------------------------------------------------------------------------------------------ launches
-# Child process: for each case [M, N, K, entry, combo] the full names of the CUDA kernels of one call, after a first call
-# outside the profiled region.  entry "linear" is w8a8_linear_forward_cuda with the combo's operands, "gemm" today's
-# w8a8_gemm[_fuse_bias]_forward_cuda.
-_PROFILE = """
-import json, sys
-sys.path[:0] = sys.argv[1:3]
-import torch
-import llm_awq_b200 as P
-import w8a8_cases as W
-eng = P.engine()
-out = []
-for M, N, K, entry, (cb, cl, cr) in json.loads(sys.argv[3]):
-    x, w, ws, a, b = W.gemm_inputs(M, N, K, "cuda")
-    ls = torch.ones(N, dtype=torch.float16, device="cuda")
-    res = torch.ones(M, N, dtype=torch.float16, device="cuda")
-    y = torch.empty(M, N, dtype=torch.float16, device="cuda")
+def traced_call(M, N, K, entry, combo):
+    """kernel_trace builder: entry "linear" is w8a8_linear_forward_cuda with the combo's operands, "gemm" today's
+    w8a8_gemm[_fuse_bias]_forward_cuda."""
+    eng = P.engine()
+    cb, cl, cr = combo
+    x, w, ws, a, b = W.gemm_inputs(M, N, K, DEV)
+    ls = torch.ones(N, dtype=F16, device=DEV)
+    res = torch.ones(M, N, dtype=F16, device=DEV)
+    y = torch.empty(M, N, dtype=F16, device=DEV)
     if entry == "linear":
-        call = lambda: eng.w8a8_linear_forward_cuda(x, w, ws, a, y, bias=b if cb else None, layer_scale=ls if cl else None,
+        return lambda: eng.w8a8_linear_forward_cuda(x, w, ws, a, y, bias=b if cb else None, layer_scale=ls if cl else None,
                                                     residual=res if cr else None)
-    elif cb:
-        call = lambda: eng.w8a8_gemm_fuse_bias_forward_cuda(x, w, ws, a, y, b)
-    else:
-        call = lambda: eng.w8a8_gemm_forward_cuda(x, w, ws, a, y)
-    call()
-    torch.cuda.synchronize()
-    c0 = eng.launch_count()
-    call()
-    torch.cuda.synchronize()
-    launches = eng.launch_count() - c0
-    for attempt in range(3):  # a session that recorded no kernel at all lost its activity records: profile again
-        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-            call()
-            torch.cuda.synchronize()
-        names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-        if names:
-            break
-    out.append([launches, names])
-print(json.dumps(out))
-"""
-
-
-def profiled_kernels(cases, per_process=16):
-    tests = os.path.dirname(os.path.abspath(__file__))
-    out = []
-    for i in range(0, len(cases), per_process):
-        r = subprocess.run([sys.executable, "-s", "-c", _PROFILE, os.path.dirname(tests), tests,
-                            json.dumps(cases[i:i + per_process])], capture_output=True, text=True, timeout=900)
-        assert r.returncode == 0, r.stderr[-3000:]
-        out += json.loads(r.stdout.strip().splitlines()[-1])
-    return out
+    if cb:
+        return lambda: eng.w8a8_gemm_fuse_bias_forward_cuda(x, w, ws, a, y, b)
+    return lambda: eng.w8a8_gemm_forward_cuda(x, w, ws, a, y)
 
 
 def test_launches_pinned_by_kernel_name():
@@ -197,7 +159,8 @@ def test_launches_pinned_by_kernel_name():
     shapes = [(1, 1152, 1152), (129, 4304, 1152), (1025, 1024, 4096), (8192, 1152, 4304)]
     cases = [[M, N, K, entry, list(c)] for M, N, K in shapes for c in COMBOS for entry in ("linear", "gemm")
              if entry == "linear" or not (c[1] or c[2])]
-    got = dict(zip([json.dumps(c) for c in cases], profiled_kernels(cases)))
+    got = {json.dumps(c): (r.launches, r.names)
+           for c, r in zip(cases, trace("test_w8a8_epilogue_gpu:traced_call", cases, per_process=16))}
     for M, N, K in shapes:
         for c in COMBOS:
             launches, names = got[json.dumps([M, N, K, "linear", list(c)])]
