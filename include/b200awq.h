@@ -123,6 +123,31 @@ int b200awq_w4a16_mlp_front(const void* x, const void* gate_qweight, const void*
                             int group_size, int dtype, void* workspace, size_t workspace_bytes, void* stream);
 size_t b200awq_w4a16_mlp_front_workspace_bytes(int m, int n, int k);
 
+/* RMSNorm prologues of the decoder's norm -> linear launches (DESIGN §3.5c): the attention block's
+ * `input_layernorm -> qkv_proj` and the MLP's `post_attention_layernorm -> gate/up`.  With x^ = the output of
+ * b200awq_rmsnorm(x, gamma, eps) (fp16 clamp included), bit for bit:
+ *   b200awq_w4a16_norm_linear(x, gamma, eps, W, bias)     == b200awq_w4a16_linear(x^, W, bias, residual = NULL)
+ *   b200awq_w4a16_norm_mlp_front(x, gamma, eps, Wg, Wu)  == b200awq_w4a16_mlp_front(x^, Wg, Wu)
+ * for every m, dtype and shape the plain entries take.  One fp16 token (and the ring kernel's m = 2..4 / bf16 m = 1 for
+ * norm_linear) computes the row statistic and x^ inside the W4A16 launch: one kernel, the plain launch's plan.  Every
+ * other shape writes x^ into the workspace with b200awq_rmsnorm and runs the plain route on it.
+ *   gamma     [k] of the activation dtype, 16-byte aligned (else B200AWQ_ERR_ALIGN); a model constant: it is read
+ *             before the dependency wait, so it must not be written by the launch right before
+ *   eps       finite and >= 0 (else B200AWQ_ERR_SHAPE)
+ *   workspace 16-byte aligned, required on every call, also when the one-kernel route needs none (else
+ *             B200AWQ_ERR_WORKSPACE): norm_linear needs m * k * 2 bytes (8 KB for one token at k = 4096), norm_mlp_front
+ *             b200awq_w4a16_norm_workspace_bytes(m, n, k) = m * k * 2 + 2 * m * n * 2, which also serves norm_linear.
+ *             It must not overlap x, y or the weights.
+ * Otherwise the return codes of b200awq_w4a16_linear / b200awq_w4a16_mlp_front.  No residual operand. */
+int b200awq_w4a16_norm_linear(const void* x, const void* gamma, float eps, const void* qweight, const void* scales,
+                              const void* szeros, const void* bias, void* y, int m, int n, int k, int group_size, int dtype,
+                              void* workspace, size_t workspace_bytes, void* stream);
+int b200awq_w4a16_norm_mlp_front(const void* x, const void* gamma, float eps, const void* gate_qweight,
+                                 const void* gate_scales, const void* gate_szeros, const void* up_qweight,
+                                 const void* up_scales, const void* up_szeros, void* y, int m, int n, int k, int group_size,
+                                 int dtype, void* workspace, size_t workspace_bytes, void* stream);
+size_t b200awq_w4a16_norm_workspace_bytes(int m, int n, int k);
+
 /* RMSNorm of the decoder layers around the quantised linears (SURVEY.md §8f-2): y[i, :] = x[i, :] *
  * rsqrt(mean(x[i, :]^2) + eps) * gamma, statistics in fp32, one rounding to the element type (fp16 results are
  * clamped to +-(65504 - 1000) like the reference).  Replaces layernorm_forward_cuda(input, gamma, out, eps)

@@ -38,7 +38,7 @@ def _run(cmd):
 
 def build_lib(force=False):
     srcs = [os.path.join(CSRC, f) for f in KERNEL_SRCS]
-    deps = srcs + [os.path.join(CSRC, f) for f in ("w4_common.cuh", "w4a16_kernels.h", "rope_neox.cuh", "rope_kv_store.cuh", "tma_wgmma.cuh", "w8a8_math.cuh",
+    deps = srcs + [os.path.join(CSRC, f) for f in ("w4_common.cuh", "w4a16_kernels.h", "rmsnorm_stat.cuh", "rope_neox.cuh", "rope_kv_store.cuh", "tma_wgmma.cuh", "w8a8_math.cuh",
                                                  "attention_wgmma.cuh")] + \
         [os.path.join(INCLUDE, "b200awq.h"), __file__]
     if not force and _newer(LIB, deps):

@@ -109,13 +109,15 @@ bool use_flat(int m, int n, int k) {
   return n % 128 == 0 && m >= min_m && m <= kFlatMaxM;
 }
 
-// One W4A16 product y = x W~^T (+ epilogue), as validated by the entry.
+// One W4A16 product y = x W~^T (+ epilogue), or x^ W~^T with x^ = RMSNorm(x) (+ epilogue), as validated by the entry.
 struct W4Operands {
   const void *x, *qw, *sc, *sz;
   void* y;
   int m, n, k, dtype;
   cudaStream_t st;
   b200awq::Epilogue epi;
+  b200awq::NormPrologue norm;  // b200awq_w4a16_norm_linear; gamma null: none
+  void* xhat = nullptr;        // with a prologue: [m, k] of workspace for x^ on the routes without one
 };
 
 // The kernels an entry may route to.
@@ -128,22 +130,59 @@ enum class Envelope {
 // Routing of every W4A16 entry.  Small token counts take decode (one fp16 token) -> ring -> flat -> stream, each returning
 // B200AWQ_ERR_SHAPE (or, for the cluster kernels, a launch-configuration error) when it cannot take the shape; outside
 // kGemv, a shape none of them takes goes to the 128-channel wgmma tiles (split-k over a cluster for small token counts).
+// An RMSNorm prologue rides along with decode and ring; before any later route, one RMSNorm launch (counted here) writes
+// x^ into o.xhat and the route reads it, which is bit-identical by construction.
 int launch_w4a16(const W4Operands& o, Envelope env) {
-  const auto& [x, qw, sc, sz, y, m, n, k, dtype, st, epi] = o;
+  const auto& [x_in, qw, sc, sz, y, m, n, k, dtype, st, epi, norm, xhat] = o;
   const bool pdl = pdl_enabled();
+  const void* x = x_in;
+  bool composed = !norm.on();
+  auto compose = [&o, &x, &composed, pdl]() {
+    if (composed) return 0;
+    composed = true;
+    x = o.xhat;
+    return counted(b200awq::launch_rmsnorm(o.x, o.norm.gamma, o.xhat, o.norm.eps, o.m, o.k, o.dtype, pdl, o.st));
+  };
   // kGemm: 9..16 tokens on the large layers (>= 48 M weights) take the persistent tile launch (split-k) directly
   const bool big_mid = env == Envelope::kGemm && m > 8 && (long long)n * k >= 48ll * 1000 * 1000;
   int r = B200AWQ_ERR_SHAPE;
   if (!big_mid) {
     if (use_decode(m, dtype))
-      r = next_on_config_error(b200awq::launch_decode(x, qw, sc, sz, y, n, k, dtype, pdl, decode_tuning(), st, epi));
-    if (r != 0 && m <= kRingMaxM) r = next_on_config_error(b200awq::launch_ring(x, qw, sc, sz, y, m, n, k, dtype, pdl, st, epi));
+      r = next_on_config_error(b200awq::launch_decode(x, qw, sc, sz, y, n, k, dtype, pdl, decode_tuning(), st, epi, norm));
+    if (r != 0 && m <= kRingMaxM)
+      r = next_on_config_error(b200awq::launch_ring(x, qw, sc, sz, y, m, n, k, dtype, pdl, st, epi, norm));
+    if (r != 0 && (use_flat(m, n, k) || m <= kStreamMaxM))
+      if (int e = compose()) return e;
     if (r != 0 && use_flat(m, n, k)) r = next_on_config_error(b200awq::launch_flat(x, qw, sc, sz, y, m, n, k, dtype, pdl, st, epi));
     if (r != 0 && m <= kStreamMaxM) r = b200awq::launch_stream(x, qw, sc, sz, y, m, n, k, dtype, pdl, st, nullptr, epi);
   }
-  if (env != Envelope::kGemv && r == B200AWQ_ERR_SHAPE && n % 128 == 0)
+  if (env != Envelope::kGemv && r == B200AWQ_ERR_SHAPE && n % 128 == 0) {
+    if (int e = compose()) return e;
     r = b200awq::launch_umma(x, qw, sc, sz, y, m, n, k, dtype, pdl, st, epi);
+  }
   return r;
+}
+
+// The RMSNorm entries' own checks, all without a device: gamma, eps and a workspace of at least `need` bytes.
+int check_norm(const void* gamma, float eps, const void* workspace, size_t workspace_bytes, size_t need) {
+  if (!aligned16(gamma)) return B200AWQ_ERR_ALIGN;
+  if (!(std::isfinite(eps) && eps >= 0.f)) return B200AWQ_ERR_SHAPE;
+  if (!aligned16(workspace) || workspace_bytes < need) return B200AWQ_ERR_WORKSPACE;
+  return 0;
+}
+
+// mlp_front's composed path: the two projections into `workspace` (2 m n elements) and silu_mul, one count per kernel
+int mlp_front_composed(const void* x, const void* gate_qweight, const void* gate_scales, const void* gate_szeros,
+                       const void* up_qweight, const void* up_scales, const void* up_szeros, void* y, int m, int n, int k,
+                       int dtype, void* workspace, cudaStream_t st) {
+  const size_t half = (size_t)m * n * 2;
+  void* g = workspace;
+  void* u = static_cast<char*>(workspace) + half;
+  const W4Operands gate{x, gate_qweight, gate_scales, gate_szeros, g, m, n, k, dtype, st};
+  const W4Operands up{x, up_qweight, up_scales, up_szeros, u, m, n, k, dtype, st};
+  for (const W4Operands* o : {&gate, &up})
+    if (int r = counted(launch_w4a16(*o, Envelope::kMlpProjection))) return r;
+  return counted(b200awq::launch_silu_mul(g, u, y, 1, (size_t)m * n, (size_t)m * n, dtype, pdl_enabled(), st));
 }
 
 // The TMA attention entries' common checks: dtype, sizes, head ratio and scale (the softmax runs on the raw scores'
@@ -231,13 +270,48 @@ int b200awq_w4a16_mlp_front(const void* x, const void* gate_qweight, const void*
     return counted(0);
   const size_t half = (size_t)m * n * 2;
   if (!workspace || workspace_bytes < 2 * half || !aligned16(workspace)) return B200AWQ_ERR_WORKSPACE;
-  void* g = workspace;
-  void* u = static_cast<char*>(workspace) + half;
-  const W4Operands gate{x, gate_qweight, gate_scales, gate_szeros, g, m, n, k, dtype, st};
-  const W4Operands up{x, up_qweight, up_scales, up_szeros, u, m, n, k, dtype, st};
-  for (const W4Operands* o : {&gate, &up})
-    if (int r = counted(launch_w4a16(*o, Envelope::kMlpProjection))) return r;
-  return counted(b200awq::launch_silu_mul(g, u, y, 1, (size_t)m * n, (size_t)m * n, dtype, pdl_enabled(), st));
+  return mlp_front_composed(x, gate_qweight, gate_scales, gate_szeros, up_qweight, up_scales, up_szeros, y, m, n, k, dtype,
+                            workspace, st);
+}
+
+size_t b200awq_w4a16_norm_workspace_bytes(int m, int n, int k) {
+  return m > 0 && n > 0 && k > 0 ? (size_t)m * k * 2 + (size_t)2 * m * n * 2 : 0;
+}
+
+int b200awq_w4a16_norm_linear(const void* x, const void* gamma, float eps, const void* qweight, const void* scales,
+                              const void* szeros, const void* bias, void* y, int m, int n, int k, int group_size, int dtype,
+                              void* workspace, size_t workspace_bytes, void* stream) {
+  if (int e = check_args(x, qweight, scales, szeros, y, m, n, k, group_size, dtype)) return e;
+  if (bias && !aligned16(bias)) return B200AWQ_ERR_ALIGN;
+  if (m >= 8 && n % 128) return B200AWQ_ERR_SHAPE;  // as b200awq_w4a16_linear
+  if (int e = check_norm(gamma, eps, workspace, workspace_bytes, (size_t)m * k * 2)) return e;
+  if (int e = check_device()) return e;
+  const W4Operands o{x,  qweight, scales, szeros, y, m, n, k, dtype, static_cast<cudaStream_t>(stream), {bias, nullptr},
+                     {gamma, eps}, workspace};
+  return counted(launch_w4a16(o, m < 8 ? Envelope::kGemv : Envelope::kGemm));
+}
+
+int b200awq_w4a16_norm_mlp_front(const void* x, const void* gamma, float eps, const void* gate_qweight,
+                                 const void* gate_scales, const void* gate_szeros, const void* up_qweight,
+                                 const void* up_scales, const void* up_szeros, void* y, int m, int n, int k, int group_size,
+                                 int dtype, void* workspace, size_t workspace_bytes, void* stream) {
+  if (int e = check_args(x, gate_qweight, gate_scales, gate_szeros, y, m, n, k, group_size, dtype)) return e;
+  if (!aligned16(up_qweight) || !aligned16(up_scales) || !aligned16(up_szeros)) return B200AWQ_ERR_ALIGN;
+  if (m >= 8 && n % 128) return B200AWQ_ERR_SHAPE;
+  if (int e = check_norm(gamma, eps, workspace, workspace_bytes, b200awq_w4a16_norm_workspace_bytes(m, n, k))) return e;
+  if (int e = check_device()) return e;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool pdl = pdl_enabled();
+  // the fused one-token kernel with the prologue, else x^ into the workspace and mlp_front's composed path behind it
+  if (use_decode(m, dtype) &&
+      next_on_config_error(b200awq::launch_decode_mlp_front(x, gate_qweight, gate_scales, gate_szeros, up_qweight, up_scales,
+                                                            up_szeros, y, n, k, dtype, pdl, decode_tuning(), st,
+                                                            {gamma, eps})) == 0)
+    return counted(0);
+  void* xhat = workspace;
+  if (int r = counted(b200awq::launch_rmsnorm(x, gamma, xhat, eps, m, k, dtype, pdl, st))) return r;
+  return mlp_front_composed(xhat, gate_qweight, gate_scales, gate_szeros, up_qweight, up_scales, up_szeros, y, m, n, k, dtype,
+                            static_cast<char*>(workspace) + (size_t)m * k * 2, st);
 }
 
 size_t b200awq_single_query_attention_workspace_bytes(int batch, int heads, int kv_heads, int head_dim, int max_len) {

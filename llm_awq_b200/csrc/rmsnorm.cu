@@ -12,46 +12,21 @@
 // the row is read ONCE with 16-byte loads and kept in registers between the reduction and the scaling (the
 // reference reads it twice with 2-byte loads); all loads of a thread are issued before the first use.  Rows wider
 // than the register budget, not a multiple of 8 elements, or on pointers that are not 16-byte aligned take the generic
-// two-pass kernel, which sums in the same order.
+// two-pass kernel, which sums in the same order.  That order, norm_round and norm_pair live in rmsnorm_stat.cuh: the
+// W4A16 decode kernels' RMSNorm prologues use the same ones, which makes them bit-identical to this kernel.
+#include "rmsnorm_stat.cuh"
 #include "w4_common.cuh"
 #include "w4a16_kernels.h"
 
 namespace b200awq {
 namespace {
 
-constexpr int kNormThreads = 256;
-
-template <typename T>
-__device__ __forceinline__ float2 pair_to_float2(uint32_t v) {
-  if constexpr (TypeTraits<T>::kIsBf16) return __bfloat1622float2(u32_as_b2(v));
-  else return __half22float2(u32_as_h2(v));
-}
-// reduction.cuh:72-82: finite clamp for fp16 only
-template <typename T>
-__device__ __forceinline__ T norm_round(float v) {
-  if constexpr (TypeTraits<T>::kIsBf16) {
-    return __float2bfloat16_rn(v);
-  } else {
-    constexpr float kLim = 65504.f - 1000.f;
-    return v > 0.f ? __float2half_rn(fminf(v, kLim)) : __float2half_rn(fmaxf(v, -kLim));
-  }
-}
-template <typename T>
-__device__ __forceinline__ uint32_t norm_pair(uint32_t x2, uint32_t g2, float r) {
-  const float2 x = pair_to_float2<T>(x2), g = pair_to_float2<T>(g2);
-  const T lo = norm_round<T>((x.x * r) * g.x), hi = norm_round<T>((x.y * r) * g.y);
-  return (uint32_t)(*reinterpret_cast<const uint16_t*>(&lo)) | ((uint32_t)(*reinterpret_cast<const uint16_t*>(&hi)) << 16);
-}
-
-__device__ __forceinline__ float block_sum(float v, float* red) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  if (lane == 0) red[warp] = v;
+// r of this CTA's row from each thread's accumulator s, in the order of rmsnorm_stat.cuh
+__device__ __forceinline__ float block_rstd(float s, float* red, int n, float eps) {
+  s = norm_warp_sum(s);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
   __syncthreads();
-  float t = 0.f;
-  for (int w = 0; w < nw; ++w) t += red[w];  // every thread, same fixed order: deterministic, no second barrier
-  return t;
+  return norm_rstd(red, n, eps);  // every thread, same fixed order: deterministic, no second barrier
 }
 
 // NCH 16-byte chunks per thread live in registers.
@@ -78,16 +53,8 @@ __global__ void __launch_bounds__(kNormThreads) rmsnorm_rows_kernel(const T* __r
   }
   float s = 0.f;
 #pragma unroll
-  for (int j = 0; j < NCH; ++j) {
-    const uint32_t w[4] = {v[j].x, v[j].y, v[j].z, v[j].w};
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const float2 p = pair_to_float2<T>(w[e]);
-      s = fmaf(p.x, p.x, s);
-      s = fmaf(p.y, p.y, s);
-    }
-  }
-  const float r = rsqrtf(block_sum(s, red) / (float)n + eps);
+  for (int j = 0; j < NCH; ++j) s = norm_chunk_sumsq<T>(v[j], s);
+  const float r = block_rstd(s, red, n, eps);
   uint4* yv = reinterpret_cast<uint4*>(y + (size_t)blockIdx.x * n);
 #pragma unroll
   for (int j = 0; j < NCH; ++j) {
@@ -99,7 +66,7 @@ __global__ void __launch_bounds__(kNormThreads) rmsnorm_rows_kernel(const T* __r
 }
 
 // any n and alignment: two passes over the row (the second one hits L1 / L2).  The sum of squares runs in the order of
-// rmsnorm_rows_kernel -- thread t owns the 8-element chunks t, t + 256, ..., each in element order -- so a row that
+// rmsnorm_stat.cuh -- thread t owns the 8-element chunks t, t + 256, ..., each in element order -- so a row that
 // either kernel can take gives the same bits on both, whatever the alignment of its pointers.
 template <typename T>
 __global__ void __launch_bounds__(kNormThreads) rmsnorm_generic_kernel(const T* __restrict__ x, const T* __restrict__ gamma,
@@ -116,7 +83,7 @@ __global__ void __launch_bounds__(kNormThreads) rmsnorm_generic_kernel(const T* 
       s = fmaf(f, f, s);
     }
   }
-  const float r = rsqrtf(block_sum(s, red) / (float)n + eps);
+  const float r = block_rstd(s, red, n, eps);
   T* yr = y + (size_t)blockIdx.x * n;
   for (int i = threadIdx.x; i < n; i += kNormThreads)
     yr[i] = norm_round<T>((to_float<T>(xr[i]) * r) * to_float<T>(gamma[i]));

@@ -151,6 +151,60 @@ torch::Tensor mlp_front_forward_cuda(torch::Tensor _in_feats, torch::Tensor _gat
   return out;
 }
 
+namespace {
+// gamma [k] of in_feats' dtype and device, contiguous (the checks of layernorm_forward_cuda); a workspace of `bytes` from
+// the caching allocator
+at::Tensor norm_workspace(const torch::Tensor& in, const torch::Tensor& gamma, int64_t k, size_t bytes, const char* fn) {
+  TORCH_CHECK(gamma.is_cuda() && gamma.device() == in.device(), fn, ": gamma must be on in_feats' device");
+  TORCH_CHECK(gamma.scalar_type() == in.scalar_type(), fn, ": gamma must have in_feats' dtype");
+  TORCH_CHECK(gamma.is_contiguous() && gamma.numel() == k, fn, ": gamma must be contiguous with ", k, " elements");
+  return torch::empty({(int64_t)std::max<size_t>(bytes, 16)}, in.options().dtype(torch::kUInt8));
+}
+}  // namespace
+
+// New entry: tinychat's `input_layernorm(x)` followed by the q/k/v projection (+ bias) in one call, bit-identical to
+// layernorm_forward_cuda followed by w4a16_linear_forward_cuda (include/b200awq.h, b200awq_w4a16_norm_linear).
+torch::Tensor rmsnorm_w4a16_linear_forward_cuda(torch::Tensor _in_feats, torch::Tensor _gamma, double eps, torch::Tensor _kernel,
+                                                torch::Tensor _scales, torch::Tensor _zeros, int64_t group_size,
+                                                c10::optional<torch::Tensor> bias) {
+  const char* fn = "rmsnorm_w4a16_linear_forward_cuda";
+  const W4Shape s = w4a16_shape(_in_feats, _kernel, _scales, _zeros, group_size, fn);
+  if (bias.has_value()) {
+    TORCH_CHECK(bias->is_cuda() && bias->device() == _in_feats.device(), fn, ": bias must be on in_feats' device");
+    TORCH_CHECK(bias->scalar_type() == _in_feats.scalar_type(), fn, ": bias must have in_feats' dtype");
+    TORCH_CHECK(bias->is_contiguous() && bias->dim() == 1 && bias->size(0) == s.n, fn, ": bias must be contiguous [", s.n, "]");
+  }
+  const c10::cuda::CUDAGuard guard(_in_feats.device());
+  const size_t bytes = (size_t)s.m * (size_t)s.k * 2;  // x^ for the routes without the prologue (include/b200awq.h)
+  const at::Tensor ws = norm_workspace(_in_feats, _gamma, s.k, bytes, fn);
+  at::Tensor out = torch::empty(s.out_shape, _in_feats.options());
+  if (s.m == 0) return out;
+  raise(b200awq_w4a16_norm_linear(_in_feats.data_ptr(), _gamma.data_ptr(), (float)eps, _kernel.data_ptr(), _scales.data_ptr(),
+                                  _zeros.data_ptr(), bias.has_value() ? bias->data_ptr() : nullptr, out.data_ptr(), (int)s.m,
+                                  (int)s.n, (int)s.k, (int)group_size, s.dt, ws.data_ptr(), bytes, current_stream()));
+  return out;
+}
+
+// New entry: tinychat's `post_attention_layernorm(x)` followed by QuantLlamaMLP.our_llama_mlp in one call, bit-identical
+// to layernorm_forward_cuda followed by mlp_front_forward_cuda (b200awq_w4a16_norm_mlp_front).
+torch::Tensor rmsnorm_mlp_front_forward_cuda(torch::Tensor _in_feats, torch::Tensor _gamma, double eps,
+                                             torch::Tensor _gate_kernel, torch::Tensor _gate_scales, torch::Tensor _gate_zeros,
+                                             torch::Tensor _up_kernel, torch::Tensor _up_scales, torch::Tensor _up_zeros) {
+  const char* fn = "rmsnorm_mlp_front_forward_cuda";
+  const W4Shape s = w4a16_shape(_in_feats, _gate_kernel, _gate_scales, _gate_zeros, 128, fn);
+  TORCH_CHECK(w4a16_shape(_in_feats, _up_kernel, _up_scales, _up_zeros, 128, fn).n == s.n, "qweights do not match");
+  const c10::cuda::CUDAGuard guard(_in_feats.device());
+  const size_t bytes = b200awq_w4a16_norm_workspace_bytes((int)s.m, (int)s.n, (int)s.k);
+  const at::Tensor ws = norm_workspace(_in_feats, _gamma, s.k, bytes, fn);
+  at::Tensor out = torch::empty(s.out_shape, _in_feats.options());
+  if (s.m == 0) return out;
+  raise(b200awq_w4a16_norm_mlp_front(_in_feats.data_ptr(), _gamma.data_ptr(), (float)eps, _gate_kernel.data_ptr(),
+                                     _gate_scales.data_ptr(), _gate_zeros.data_ptr(), _up_kernel.data_ptr(),
+                                     _up_scales.data_ptr(), _up_zeros.data_ptr(), out.data_ptr(), (int)s.m, (int)s.n, (int)s.k,
+                                     128, s.dt, ws.data_ptr(), bytes, current_stream()));
+  return out;
+}
+
 // reference: awq/kernels/csrc/layernorm/layernorm.cu:111-131 (input [b, s, c], gamma [c], out like input; returns
 // nothing).  Same dtype checks; additionally any rank >= 1 is accepted (rows = numel / last dim), the launch goes to
 // the current stream, and contiguity is checked instead of assumed.
@@ -691,6 +745,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("scales"), py::arg("zeros"), py::arg("group_size"), py::arg("bias") = py::none(),
         py::arg("residual") = py::none());
   m.def("mlp_front_forward_cuda", &mlp_front_forward_cuda, "silu(x Wgate^T) * (x Wup^T) for W4A16 weights, one call");
+  m.def("rmsnorm_w4a16_linear_forward_cuda", &rmsnorm_w4a16_linear_forward_cuda,
+        "RMSNorm(x) W^T (+ bias) for W4A16 weights, bit-identical to layernorm_forward_cuda + w4a16_linear_forward_cuda",
+        py::arg("in_feats"), py::arg("gamma"), py::arg("eps"), py::arg("kernel"), py::arg("scales"), py::arg("zeros"),
+        py::arg("group_size"), py::arg("bias") = py::none());
+  m.def("rmsnorm_mlp_front_forward_cuda", &rmsnorm_mlp_front_forward_cuda,
+        "silu(RMSNorm(x) Wgate^T) * (RMSNorm(x) Wup^T), bit-identical to layernorm_forward_cuda + mlp_front_forward_cuda",
+        py::arg("in_feats"), py::arg("gamma"), py::arg("eps"), py::arg("gate_kernel"), py::arg("gate_scales"),
+        py::arg("gate_zeros"), py::arg("up_kernel"), py::arg("up_scales"), py::arg("up_zeros"));
   m.def("w8a8_gemm_forward_cuda", &w8a8_gemm_forward_cuda, "our w8a8 gemm kernel");
   m.def("w8a8_gemm_fuse_bias_forward_cuda", &w8a8_gemm_fuse_bias_forward_cuda, "our w8a8 gemm fused bias kernel");
   m.def("w8a8_linear_forward_cuda", &w8a8_linear_forward_cuda,

@@ -38,6 +38,7 @@
 // touched after the wait.
 #include <algorithm>
 
+#include "rmsnorm_stat.cuh"
 #include "w4_common.cuh"
 #include "w4a16_kernels.h"
 
@@ -118,6 +119,8 @@ struct DecArgs {
   DecLayout L;
   const void* bias;      // EPI: [N] or null
   const void* residual;  // EPI: [1, N] or null
+  const void* gamma;     // NORM: [K], the RMSNorm weight applied to x before the product
+  float eps;             // NORM
 };
 
 __device__ __forceinline__ void dec_sts8(uint32_t addr, int v) {
@@ -142,8 +145,14 @@ __device__ __forceinline__ T silu_mul_rounded(float gate_acc, float up_acc) {
 // FUSED = false: y = x W~^T.   FUSED = true: y = silu(x Wgate~^T) * (x Wup~^T), both weight sets walked row block by row
 // block through the same ring (SURVEY.md §8f-1: one read of x, two weight streams, one [1, n] write).
 // EPI (not with FUSED): the finisher adds a.bias / a.residual to each stored value (add_epilogue).
-template <bool FUSED, bool EPI>
-__global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(const __grid_constant__ DecArgs a) {
+// NORM: the product reads x^ = RMSNorm(x, a.gamma, a.eps) instead of x, bit-identical to rmsnorm.cu's output (DESIGN
+// §3.5c): consumer warps 0-7 play the 256 threads of rmsnorm_stat.cuh's summation order over the whole row (also with
+// k split over the cluster), park the 8 warp totals in rank 0's `hold` area (which the finisher first writes after all
+// 16 consumer warps have arrived on rbfull[0]), and every consumer warp normalises the values it stages.
+// The body is shared by two kernel names: w4a16_decode_kernel<FUSED, EPI> (NORM = false, the names the plain entries
+// have always launched) and w4a16_decode_norm_kernel<FUSED, EPI> (NORM = true).
+template <bool FUSED, bool EPI, bool NORM>
+__device__ __forceinline__ void decode_body(const DecArgs& a) {
   static_assert(!(FUSED && EPI), "the fused MLP front has no epilogue");
   using T = __half;
   constexpr int NT = FUSED ? 2 : 1;   // weight sets
@@ -315,14 +324,24 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
   constexpr int kMaxOwn = 32 / kDecCons;  // groups a warp converts together (k = 4096: all of its groups)
   const int x_eoff = (lane >> 3) * 32 + ((lane >> 2) & 1) * 8 + 2 * (lane & 3);  // see the digit staging below
   const uint32_t* xfirst[kMaxOwn];
+  uint32_t ga0[kMaxOwn], gb0[kMaxOwn];  // NORM: gamma of the first batch, a model constant: loaded before the wait
 #pragma unroll
   for (int i = 0; i < kMaxOwn; ++i) {
     const int Gl = min(warp + i * kDecCons, max(ngr - 1, 0));
     xfirst[i] = reinterpret_cast<const uint32_t*>(reinterpret_cast<const T*>(a.x) + (size_t)(kg_lo + Gl) * kGroup + x_eoff);
+    if (NORM && warp < kDecCons) {
+      const uint32_t* gf =
+          reinterpret_cast<const uint32_t*>(static_cast<const T*>(a.gamma) + (size_t)(kg_lo + Gl) * kGroup + x_eoff);
+      ga0[i] = __ldg(gf), gb0[i] = __ldg(gf + 8);
+    }
   }
+  constexpr int kNormFirst = 4;  // chunks per statistic thread loaded before the first use: all of them up to k = 8192
+  uint4 nv[kNormFirst];
   pdl_wait_prior_grid();  // activations (and y) belong to the stream order from here on
   uint32_t xa0[kMaxOwn], xb0[kMaxOwn];
   if (warp < kDecCons) {
+    // NORM: the statistic's row loads first, then this warp's first batch; nothing is used before all are issued
+    if (NORM && warp < kNormWarps) norm_first_chunks<T, kNormFirst>(static_cast<const T*>(a.x), K, warp * 32 + lane, nv);
 #pragma unroll
     for (int i = 0; i < kMaxOwn; ++i) {
       asm volatile("ld.global.u32 %0, [%1];" : "=r"(xa0[i]) : "l"(xfirst[i]) : "memory");
@@ -414,6 +433,16 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
   const int c = lane >> 2, tig = lane & 3;
   const uint32_t xd_u32 = smem_u32(smem + L.x);
   float* gx = reinterpret_cast<float*>(smem + L.gx);  // [group][tig]: e_g 2^-7 tig / 16 for the digit lanes tig < 3, X_g = sum_k x_k for tig 3
+  float rstd = 0.f;  // NORM: r of the row
+  if constexpr (NORM) {
+    float* nstat = xchg + (S - 1) * a.nrb_max * RW;  // rank 0's `hold` area, unused until the first row block is summed
+    if (warp < kNormWarps) {
+      const float s = norm_warp_sum(norm_thread_sumsq<T, kNormFirst>(nv, static_cast<const T*>(a.x), K, warp * 32 + lane));
+      if (lane == 0) nstat[warp] = s;
+    }
+    asm volatile("bar.sync 1, %0;" ::"n"(kDecCons * 32) : "memory");  // the consumer warps only
+    rstd = norm_rstd(nstat, K, a.eps);
+  }
   {
     // Digits.  A digit word [column 2 d + par][u][m] (par 0: low-nibble channels, 1: high-nibble channels) holds the
     // four input channels m * 32 + par * 8 + {0, 16} + 2 u + {0, 1} of the group (see the packed layout in
@@ -431,10 +460,16 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
       for (int i = 0; i < kMaxOwn; ++i) {
         if (G0 == warp) {  // the first batch was loaded right behind the dependency wait
           xa[i] = xa0[i], xb[i] = xb0[i];
+          if (NORM) xa[i] = norm_pair<T>(xa[i], ga0[i], rstd), xb[i] = norm_pair<T>(xb[i], gb0[i], rstd);
         } else {
           const int Gl = min(G0 + i * kDecCons, ngr - 1);  // clamped: the extra conversions are not stored
           const uint32_t* src = reinterpret_cast<const uint32_t*>(xg + (size_t)Gl * kGroup + eoff);
           xa[i] = src[0], xb[i] = src[8];
+          if (NORM) {
+            const uint32_t* gs =
+                reinterpret_cast<const uint32_t*>(static_cast<const T*>(a.gamma) + (size_t)(kg_lo + Gl) * kGroup + eoff);
+            xa[i] = norm_pair<T>(xa[i], __ldg(gs), rstd), xb[i] = norm_pair<T>(xb[i], __ldg(gs + 8), rstd);
+          }
         }
       }
 #pragma unroll
@@ -590,11 +625,28 @@ __global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(co
   if (warp == 0) DEC_TRACE(a.qw, kTrLastMac);
 }
 
+template <bool FUSED, bool EPI>
+__global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_kernel(const __grid_constant__ DecArgs a) {
+  decode_body<FUSED, EPI, false>(a);
+}
+
+template <bool FUSED, bool EPI>
+__global__ void __launch_bounds__((kDecCons + 2) * 32, 2) w4a16_decode_norm_kernel(const __grid_constant__ DecArgs a) {
+  decode_body<FUSED, EPI, true>(a);
+}
+
 // ------------------------------------------------------------------------------------ host
 namespace {
+template <bool FUSED, bool EPI, bool NORM>
+int launch_decode_t(const DecArgs& a, dim3 grid, dim3 block, bool pdl, cudaStream_t stream) {
+  constexpr auto kern = NORM ? w4a16_decode_norm_kernel<FUSED, EPI> : w4a16_decode_kernel<FUSED, EPI>;
+  if (cudaError_t e = ensure_dyn_smem<kern>(kDecSmemBudget, true)) return (int)e;
+  return launch_kernel(kern, grid, block, (size_t)a.L.total, stream, pdl, (unsigned)a.S, a);
+}
+
 int launch_decode_impl(const void* x, const void* qw, const void* sc, const void* sz, const void* qw2, const void* sc2,
                        const void* sz2, void* y, int N, int K, int dtype, bool pdl, const DecodeTuning& tune, cudaStream_t stream,
-                       const Epilogue& epi) {
+                       const Epilogue& epi, const NormPrologue& norm) {
   const bool fused = qw2 != nullptr;
   const int nt = fused ? 2 : 1;
   if (dtype != B200AWQ_DTYPE_F16 || N % 8 || K % kGroup) return B200AWQ_ERR_SHAPE;
@@ -605,6 +657,7 @@ int launch_decode_impl(const void* x, const void* qw, const void* sc, const void
   a.x = x, a.qw = static_cast<const uint16_t*>(qw), a.sc = sc, a.sz = sz, a.y = y;
   a.qw2 = static_cast<const uint16_t*>(qw2), a.sc2 = sc2, a.sz2 = sz2;
   a.bias = epi.bias, a.residual = epi.residual;
+  a.gamma = norm.gamma, a.eps = norm.eps;
   a.N = N, a.K = K;
   // k split: only when the rows alone cannot balance the SMs (efficiency of dealing Q quad rows to nsm CTAs below
   // ~0.9) and the halves still make copies of >= 4 KB; or when the digits of the whole k range would crowd out the ring
@@ -649,29 +702,25 @@ int launch_decode_impl(const void* x, const void* qw, const void* sc, const void
   L.total = off + ns * kDecSlotBytes;
 
   const dim3 grid((unsigned)(a.units * a.S)), block((unsigned)((kDecCons + 2) * 32));
-  if (fused) {
-    if (cudaError_t e = ensure_dyn_smem<w4a16_decode_kernel<true, false>>(kDecSmemBudget, true)) return (int)e;
-    return launch_kernel(w4a16_decode_kernel<true, false>, grid, block, (size_t)L.total, stream, pdl, (unsigned)a.S, a);
-  }
-  if (epi.on()) {
-    if (cudaError_t e = ensure_dyn_smem<w4a16_decode_kernel<false, true>>(kDecSmemBudget, true)) return (int)e;
-    return launch_kernel(w4a16_decode_kernel<false, true>, grid, block, (size_t)L.total, stream, pdl, (unsigned)a.S, a);
-  }
-  if (cudaError_t e = ensure_dyn_smem<w4a16_decode_kernel<false, false>>(kDecSmemBudget, true)) return (int)e;
-  return launch_kernel(w4a16_decode_kernel<false, false>, grid, block, (size_t)L.total, stream, pdl, (unsigned)a.S, a);
+  if (fused) return norm.on() ? launch_decode_t<true, false, true>(a, grid, block, pdl, stream)
+                              : launch_decode_t<true, false, false>(a, grid, block, pdl, stream);
+  if (epi.on()) return norm.on() ? launch_decode_t<false, true, true>(a, grid, block, pdl, stream)
+                                 : launch_decode_t<false, true, false>(a, grid, block, pdl, stream);
+  return norm.on() ? launch_decode_t<false, false, true>(a, grid, block, pdl, stream)
+                   : launch_decode_t<false, false, false>(a, grid, block, pdl, stream);
 }
 }  // namespace
 
 int launch_decode(const void* x, const void* qw, const void* sc, const void* sz, void* y, int N, int K, int dtype, bool pdl,
-                  const DecodeTuning& tune, cudaStream_t stream, const Epilogue& epi) {
-  return launch_decode_impl(x, qw, sc, sz, nullptr, nullptr, nullptr, y, N, K, dtype, pdl, tune, stream, epi);
+                  const DecodeTuning& tune, cudaStream_t stream, const Epilogue& epi, const NormPrologue& norm) {
+  return launch_decode_impl(x, qw, sc, sz, nullptr, nullptr, nullptr, y, N, K, dtype, pdl, tune, stream, epi, norm);
 }
 
 int launch_decode_mlp_front(const void* x, const void* gqw, const void* gsc, const void* gsz, const void* uqw, const void* usc,
                             const void* usz, void* y, int N, int K, int dtype, bool pdl, const DecodeTuning& tune,
-                            cudaStream_t stream) {
+                            cudaStream_t stream, const NormPrologue& norm) {
   if (!uqw || !usc || !usz) return B200AWQ_ERR_ALIGN;
-  return launch_decode_impl(x, gqw, gsc, gsz, uqw, usc, usz, y, N, K, dtype, pdl, tune, stream, Epilogue{});
+  return launch_decode_impl(x, gqw, gsc, gsz, uqw, usc, usz, y, N, K, dtype, pdl, tune, stream, Epilogue{}, norm);
 }
 
 }  // namespace b200awq

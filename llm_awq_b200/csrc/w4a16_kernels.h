@@ -96,6 +96,16 @@ struct Epilogue {
   bool on() const { return bias || residual; }
 };
 
+// RMSNorm prologue of a one-token / few-token W4A16 launch (b200awq_w4a16_norm_linear, b200awq_w4a16_norm_mlp_front):
+// the kernel multiplies x^ = RMSNorm(x, gamma, eps) (rmsnorm_stat.cuh), bit-identical to launch_rmsnorm's output, instead
+// of x.  Only launch_decode, launch_decode_mlp_front and launch_ring take one; with gamma null (the default) they launch
+// the instantiation the other entries run.
+struct NormPrologue {
+  const void* gamma = nullptr;  // [K] of the activation dtype, 16-byte aligned
+  float eps = 0.f;
+  bool on() const { return gamma != nullptr; }
+};
+
 // HBM-bound streaming kernel, 1 <= M <= 16 (w4a16_stream.cu); the epilogue does not apply to the all-reduce (peers)
 int launch_stream(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
                   bool pdl, cudaStream_t stream, const PeerArgs* peers = nullptr, const Epilogue& epi = Epilogue{});
@@ -107,7 +117,7 @@ int launch_umma(const void* x, const void* qw, const void* sc, const void* sz, v
 // persistent warp-specialised decode kernel, 1 <= M <= 4 (w4a16_ring.cu); returns B200AWQ_ERR_SHAPE when the
 // activations do not fit next to a useful ring (the caller falls back to the kernels below)
 int launch_ring(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                bool pdl, cudaStream_t stream, const Epilogue& epi = Epilogue{});
+                bool pdl, cudaStream_t stream, const Epilogue& epi = Epilogue{}, const NormPrologue& norm = NormPrologue{});
 
 // Test-only override of the decode kernel's plan (env B200AWQ_DECODE_SPLIT / B200AWQ_DECODE_SLOTS, api.cu): the
 // default-constructed value means "pick from the shape".
@@ -119,12 +129,13 @@ struct DecodeTuning {
 // one-token fp16 decode kernel: 8 KB bulk copies, int8-digit tensor-core MACs (w4a16_decode.cu); returns
 // B200AWQ_ERR_SHAPE for bf16 and when the activations do not fit next to a useful ring (the caller falls back)
 int launch_decode(const void* x, const void* qw, const void* sc, const void* sz, void* y, int N, int K, int dtype, bool pdl,
-                  const DecodeTuning& tune, cudaStream_t stream, const Epilogue& epi = Epilogue{});
+                  const DecodeTuning& tune, cudaStream_t stream, const Epilogue& epi = Epilogue{},
+                  const NormPrologue& norm = NormPrologue{});
 
 // one-token fused MLP front half: y = silu(x Wgate~^T) * (x Wup~^T), both weight sets through one ring (w4a16_decode.cu)
 int launch_decode_mlp_front(const void* x, const void* gqw, const void* gsc, const void* gsz, const void* uqw, const void* usc,
                             const void* usz, void* y, int N, int K, int dtype, bool pdl, const DecodeTuning& tune,
-                            cudaStream_t stream);
+                            cudaStream_t stream, const NormPrologue& norm = NormPrologue{});
 
 // out = silu(gate) * up over rows x cols elements, the reference's roundings; gate / up rows are in_pitch elements
 // apart, out is dense (silu_mul.cu)

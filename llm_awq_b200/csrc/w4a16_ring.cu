@@ -34,6 +34,7 @@
 // x and y are only touched after the wait.
 #include <algorithm>
 
+#include "rmsnorm_stat.cuh"
 #include "w4_common.cuh"
 #include "w4a16_kernels.h"
 
@@ -68,6 +69,8 @@ struct RingArgs {
   RingLayout L;
   const void* bias;      // EPI: [N] or null
   const void* residual;  // EPI: [M, N] or null
+  const void* gamma;     // NORM: [K], the RMSNorm weight applied to every token row of x before the product
+  float eps;             // NORM
 };
 
 __device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 1, %0;" ::"n"(kRingCons * 32) : "memory"); }
@@ -139,8 +142,13 @@ __device__ __forceinline__ void group_step(uint32_t wsrc, uint32_t xsrc, uint32_
 }
 
 // EPI: the finisher adds a.bias / a.residual to each stored value (add_epilogue)
-template <typename T, bool M1, bool EPI>
-__global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __grid_constant__ RingArgs a) {
+// NORM: the product reads x^ = RMSNorm(x, a.gamma, a.eps) instead of x, bit-identical to rmsnorm.cu's output (DESIGN
+// §3.5c).  The 256 consumer threads ARE the 256 threads of rmsnorm_stat.cuh's summation order: each token row's 8 warp
+// totals go through `red` (first written after the staging barrier), and the staging normalises every chunk it copies.
+// The body is shared by two kernel names: w4a16_ring_kernel<T, M1, EPI> (NORM = false, the names the plain entries have
+// always launched) and w4a16_ring_norm_kernel<T, M1, EPI> (NORM = true).
+template <typename T, bool M1, bool EPI, bool NORM>
+__device__ __forceinline__ void ring_body(const RingArgs& a) {
   constexpr int MODE = TypeTraits<T>::kIsBf16 ? 0 : 2;  // see the header comment
   extern __shared__ __align__(128) uint8_t smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -228,6 +236,9 @@ __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __gri
   }
 
   if (S > 1) cluster_wait();
+  // NORM: gamma of this thread's first staging chunk, a model constant: loaded before the wait
+  const uint4* gam = reinterpret_cast<const uint4*>(static_cast<const T*>(a.gamma) + (size_t)kg_lo * kGroup);
+  const uint4 g_first = NORM && warp < kRingCons && tid < ngr * 16 ? __ldg(gam + tid) : make_uint4(0u, 0u, 0u, 0u);
   pdl_wait_prior_grid();  // activations (and y) belong to the stream order from here on
 
   if (warp == kRingCons + kRingProd) {
@@ -280,6 +291,27 @@ __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __gri
   const int xrow = L.xrow;
   uint8_t* xbuf = smem + L.x;                                 // [token][group][tig][m][j] pairs (see header)
   float2* xsum = reinterpret_cast<float2*>(smem + L.xsum);    // [8 tokens][L.ngr] {X, C}
+  float rstd[4] = {0.f, 0.f, 0.f, 0.f};                        // NORM: r of each token row
+  if constexpr (NORM) {
+    constexpr int kNormFirst = 2;  // chunks per token and thread loaded before the first use: all of them up to k = 4096
+    constexpr int kTok = M1 ? 1 : 4;
+    const T* x0 = static_cast<const T*>(a.x);
+    uint4 nv[kTok][kNormFirst];
+#pragma unroll
+    for (int tok = 0; tok < kTok; ++tok)
+      if (tok < M) norm_first_chunks<T, kNormFirst>(x0 + (size_t)tok * K, K, tid, nv[tok]);
+#pragma unroll
+    for (int tok = 0; tok < kTok; ++tok) {
+      if (tok < M) {
+        const float s = norm_warp_sum(norm_thread_sumsq<T, kNormFirst>(nv[tok], x0 + (size_t)tok * K, K, tid));
+        if (lane == 0) red[tok * kNormWarps + warp] = s;
+      }
+    }
+    consumer_bar();
+#pragma unroll
+    for (int tok = 0; tok < kTok; ++tok)
+      if (tok < M) rstd[tok] = norm_rstd(red + tok * kNormWarps, K, a.eps);
+  }
   {
     // stage the activations of this rank's k range in fragment order, and the per-group sums (MODE 2)
     const T* xg = reinterpret_cast<const T*>(a.x) + (size_t)kg_lo * kGroup;
@@ -290,6 +322,15 @@ __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __gri
         const bool ok = c < nchunk;
         uint4 v = make_uint4(0, 0, 0, 0);
         if (ok) v = *reinterpret_cast<const uint4*>(xg + (size_t)tok * K + (size_t)c * 8);
+        if (NORM && ok) {
+          const uint4 gv = c0 == 0 ? g_first : __ldg(gam + c);
+          float r = rstd[0];
+#pragma unroll
+          for (int i = 1; i < 4; ++i)
+            if (!M1 && tok == i) r = rstd[i];
+          v = make_uint4(norm_pair<T>(v.x, gv.x, r), norm_pair<T>(v.y, gv.y, r), norm_pair<T>(v.z, gv.z, r),
+                         norm_pair<T>(v.w, gv.w, r));
+        }
         // chunk c holds k = 8c .. 8c+7 = the four word-pairs u = 0..3 of (32-k block m = (c & 15) >> 2, nibble pair
         // j = c & 3): lane tig = u reads it at [tig][m * 4 + j]
         if (ok) {
@@ -375,27 +416,44 @@ __global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __gri
   }
 }
 
+template <typename T, bool M1, bool EPI>
+__global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_kernel(const __grid_constant__ RingArgs a) {
+  ring_body<T, M1, EPI, false>(a);
+}
+
+template <typename T, bool M1, bool EPI>
+__global__ void __launch_bounds__(kRingThreads, 2) w4a16_ring_norm_kernel(const __grid_constant__ RingArgs a) {
+  ring_body<T, M1, EPI, true>(a);
+}
+
 // ------------------------------------------------------------------------------------ host
 namespace {
 
 constexpr int kRingSmemBudget = 113 * 1024;  // two CTAs (+ 1 KB reserved each) per 228 KB SM
 
-template <typename T, bool M1, bool EPI>
+template <typename T, bool M1, bool EPI, bool NORM>
 int launch_ring_t(const RingArgs& a, bool pdl, cudaStream_t stream) {
-  if (cudaError_t e = ensure_dyn_smem<w4a16_ring_kernel<T, M1, EPI>>(kRingSmemBudget, true)) return (int)e;
-  return launch_kernel(w4a16_ring_kernel<T, M1, EPI>, dim3((unsigned)(a.units * a.S)), dim3(kRingThreads), (size_t)a.L.total,
-                       stream, pdl, (unsigned)a.S, a);
+  constexpr auto kern = NORM ? w4a16_ring_norm_kernel<T, M1, EPI> : w4a16_ring_kernel<T, M1, EPI>;
+  if (cudaError_t e = ensure_dyn_smem<kern>(kRingSmemBudget, true)) return (int)e;
+  return launch_kernel(kern, dim3((unsigned)(a.units * a.S)), dim3(kRingThreads),
+                       (size_t)a.L.total, stream, pdl, (unsigned)a.S, a);
 }
 
-template <typename T, bool EPI>
+template <typename T, bool EPI, bool NORM>
 int launch_ring_m(const RingArgs& a, bool pdl, cudaStream_t stream) {
-  return a.M == 1 ? launch_ring_t<T, true, EPI>(a, pdl, stream) : launch_ring_t<T, false, EPI>(a, pdl, stream);
+  return a.M == 1 ? launch_ring_t<T, true, EPI, NORM>(a, pdl, stream) : launch_ring_t<T, false, EPI, NORM>(a, pdl, stream);
+}
+
+template <typename T>
+int launch_ring_dt(const RingArgs& a, bool epi, bool norm, bool pdl, cudaStream_t stream) {
+  if (norm) return epi ? launch_ring_m<T, true, true>(a, pdl, stream) : launch_ring_m<T, false, true>(a, pdl, stream);
+  return epi ? launch_ring_m<T, true, false>(a, pdl, stream) : launch_ring_m<T, false, false>(a, pdl, stream);
 }
 
 }  // namespace
 
 int launch_ring(const void* x, const void* qw, const void* sc, const void* sz, void* y, int M, int N, int K, int dtype,
-                bool pdl, cudaStream_t stream, const Epilogue& epi) {
+                bool pdl, cudaStream_t stream, const Epilogue& epi, const NormPrologue& norm) {
   if (M < 1 || M > 4 || N % 8 || K % kGroup) return B200AWQ_ERR_SHAPE;
   const int nsm = sm_count();
   if (nsm == 0) return B200AWQ_ERR_DEVICE;
@@ -404,6 +462,7 @@ int launch_ring(const void* x, const void* qw, const void* sc, const void* sz, v
   RingArgs a{};
   a.x = x, a.qw = static_cast<const uint16_t*>(qw), a.sc = sc, a.sz = sz, a.y = y;
   a.bias = epi.bias, a.residual = epi.residual;
+  a.gamma = norm.gamma, a.eps = norm.eps;
   a.M = M, a.N = N, a.K = K;
   a.S = (G >= 2 * kRingCons && nsm % 2 == 0) ? 2 : 1;
   a.units = nsm / a.S;
@@ -428,9 +487,8 @@ int launch_ring(const void* x, const void* qw, const void* sc, const void* sz, v
   if (ns < 3) return B200AWQ_ERR_SHAPE;  // activations too large next to a useful ring: the caller falls back
   a.NS = ns;
   L.total = off + ns * kSlotBytes;
-  if (dtype == B200AWQ_DTYPE_F16)
-    return epi.on() ? launch_ring_m<__half, true>(a, pdl, stream) : launch_ring_m<__half, false>(a, pdl, stream);
-  return epi.on() ? launch_ring_m<__nv_bfloat16, true>(a, pdl, stream) : launch_ring_m<__nv_bfloat16, false>(a, pdl, stream);
+  if (dtype == B200AWQ_DTYPE_F16) return launch_ring_dt<__half>(a, epi.on(), norm.on(), pdl, stream);
+  return launch_ring_dt<__nv_bfloat16>(a, epi.on(), norm.on(), pdl, stream);
 }
 
 }  // namespace b200awq

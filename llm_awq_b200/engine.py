@@ -40,6 +40,12 @@ def lib() -> ctypes.CDLL:
         L.b200awq_w4a16_mlp_front_workspace_bytes.argtypes = [ci, ci, ci]
         L.b200awq_w4a16_mlp_front_workspace_bytes.restype = sz
         ll, fl = ctypes.c_longlong, ctypes.c_float
+        L.b200awq_w4a16_norm_linear.argtypes = [vp, vp, fl, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp, sz, vp]
+        L.b200awq_w4a16_norm_linear.restype = ci
+        L.b200awq_w4a16_norm_mlp_front.argtypes = [vp, vp, fl, vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp, sz, vp]
+        L.b200awq_w4a16_norm_mlp_front.restype = ci
+        L.b200awq_w4a16_norm_workspace_bytes.argtypes = [ci, ci, ci]
+        L.b200awq_w4a16_norm_workspace_bytes.restype = sz
         L.b200awq_single_query_attention.argtypes = [vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ll, ll, ll, ci, fl, fl, ci, ci,
                                                      vp, sz, vp]
         L.b200awq_single_query_attention.restype = ci

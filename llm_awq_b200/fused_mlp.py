@@ -31,13 +31,22 @@ class QuantLlamaMLP(nn.Module):
         self.split_k_iters = down_proj.split_k_iters
         self.legacy_gemm_zero_offset = legacy_gemm_zero_offset
 
-    def forward(self, x):
-        return self.down_proj(self.our_llama_mlp(x))
+    def forward(self, x, norm=None):
+        """down_proj(our_llama_mlp(x)); norm = (weight, eps), the decoder's `post_attention_layernorm` in front of the
+        MLP, applied inside the front half's call (our_llama_mlp)."""
+        return self.down_proj(self.our_llama_mlp(x, norm))
 
-    def our_llama_mlp(self, x):
+    def our_llama_mlp(self, x, norm=None):
+        """silu(x Wgate~^T) * (x Wup~^T), or the same of RMSNorm(x) with norm = (weight, eps): bit-identical to
+        `layernorm_forward_cuda` followed by the call without it; one fp16 token normalises inside the fused kernel."""
         gz, uz = self.gate_proj_scaled_zeros, self.up_proj_scaled_zeros
         if self.legacy_gemm_zero_offset and x.numel() // x.shape[-1] >= 8:   # fused_mlp.py:69,76
             gz, uz = gz - 8 * self.gate_proj_scales, uz - 8 * self.up_proj_scales
+        if norm is not None:
+            weight, eps = norm
+            return engine().rmsnorm_mlp_front_forward_cuda(x, weight, float(eps), self.gate_proj_qweight,
+                                                           self.gate_proj_scales, gz, self.up_proj_qweight,
+                                                           self.up_proj_scales, uz)
         return engine().mlp_front_forward_cuda(x, self.gate_proj_qweight, self.gate_proj_scales, gz,
                                                self.up_proj_qweight, self.up_proj_scales, uz)
 

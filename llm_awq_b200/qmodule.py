@@ -149,6 +149,20 @@ class WQLinear(nn.Module):
             out = eng.gemm_forward_cuda_new(inputs, self.qweight, self.scales, self.scaled_zeros)
         return out + self.bias if self.bias is not None else out
 
+    @torch.no_grad()
+    def norm_forward(self, x, norm):
+        """RMSNorm(x) W~^T (+ bias) with norm = (weight, eps), the decoder's RMSNorm in front of this projection
+        (`input_layernorm` before q/k/v); norm=None is forward(x).  Bit-identical to `layernorm_forward_cuda` followed
+        by forward(); one fp16 token (and up to 4 tokens, or one bf16 token) normalises inside the W4A16 launch.
+        (A method of its own rather than a `norm` argument of forward(): forward's parameters (x, residual) are part
+        of this module's tested interface.  There is no norm + residual route.)"""
+        if norm is None:
+            return self.forward(x)
+        weight, eps = norm
+        inputs = x if x.is_contiguous() else x.contiguous()
+        return _get_engine().rmsnorm_w4a16_linear_forward_cuda(inputs, weight, float(eps), self.qweight, self.scales,
+                                                               self.scaled_zeros, self.group_size, bias=self.bias)
+
     def extra_repr(self) -> str:
         return "in_features={}, out_features={}, bias={}, w_bit={}, group_size={}".format(
             self.in_features, self.out_features, self.bias is not None, self.w_bit, self.group_size)
