@@ -183,10 +183,10 @@ prefill_attention_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_
     const uint32_t k_addr = smem_u32(kvs + stage * C::kStageBytes);
 #pragma unroll
     for (int kk = 0; kk < C::kMain / 16; ++kk)  // k16 step kk: block kk / 4, +32 bytes per step inside the block
-      wgmma_qk<T>(sc, make_smem_desc(q_addr + (kk / 4) * kBM * 128 + (kk % 4) * 32, 1, 16, 1024),
+      wgmma_ss<T>(sc, make_smem_desc(q_addr + (kk / 4) * kBM * 128 + (kk % 4) * 32, 1, 16, 1024),
                   make_smem_desc(k_addr + (kk / 4) * kBN * 128 + (kk % 4) * 32, 1, 16, 1024), kk > 0 ? 1u : 0u);
     if constexpr (C::kTail)
-      wgmma_qk<T>(sc, make_smem_desc(qt_addr, 3, 16, 256), make_smem_desc(k_addr + C::kMain * kBN * 2, 3, 16, 256), 1u);
+      wgmma_ss<T>(sc, make_smem_desc(qt_addr, 3, 16, 256), make_smem_desc(k_addr + C::kMain * kBN * 2, 3, 16, 256), 1u);
   };
   auto issue_pv = [&](int stage) {
     const uint32_t v_addr = smem_u32(kvs + stage * C::kStageBytes + C::kKBytes);
@@ -194,10 +194,10 @@ prefill_attention_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_
     float(&o_main)[C::kMain / 2] = *reinterpret_cast<float(*)[C::kMain / 2]>(o);
 #pragma unroll
     for (int kk = 0; kk < kBN / 16; ++kk) {
-      wgmma_pv<T, C::kMain>(o_main, pa[kk], make_smem_desc(v_addr + kk * 16 * 128, 1, kBN * 128, 1024), 1u);
+      wgmma_rs<T, C::kMain, true>(o_main, pa[kk], make_smem_desc(v_addr + kk * 16 * 128, 1, kBN * 128, 1024), 1u);
       if constexpr (C::kTail)
-        wgmma_pv<T, 16>(*reinterpret_cast<float(*)[8]>(o + C::kMain / 2), pa[kk],
-                        make_smem_desc(v_addr + C::kMain * kBN * 2 + kk * 16 * 32, 3, kBN * 32, 256), 1u);
+        wgmma_rs<T, 16, true>(*reinterpret_cast<float(*)[8]>(o + C::kMain / 2), pa[kk],
+                              make_smem_desc(v_addr + C::kMain * kBN * 2 + kk * 16 * 32, 3, kBN * 32, 256), 1u);
     }
   };
   // mask and online softmax of tile n's S: P into pa, O rescaled

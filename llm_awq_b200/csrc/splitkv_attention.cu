@@ -208,7 +208,7 @@ splitkv_attention_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_
     // FT K: no swizzle, 8-column blocks kBN * 16 bytes apart (two per k16 step), 8-key groups 128 bytes apart
 #pragma unroll
     for (int kk = 0; kk < D / 16; ++kk)  // k16 step kk: block kk / 4, +32 bytes per step inside the block
-      wgmma_qk<T>(sc, make_smem_desc(q_addr + (kk / 4) * kRows * 128 + (kk % 4) * 32, 1, 16, 1024),
+      wgmma_ss<T>(sc, make_smem_desc(q_addr + (kk / 4) * kRows * 128 + (kk % 4) * 32, 1, 16, 1024),
                   kFtK ? make_smem_desc(k_addr + kk * 2 * kBN * 16, 0, kBN * 16, 128)
                        : make_smem_desc(k_addr + (kk / 4) * kBN * 128 + (kk % 4) * 32, 1, 16, 1024),
                   kk > 0 ? 1u : 0u);
@@ -218,7 +218,7 @@ splitkv_attention_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_
     // V is MN-major: 64-column blocks kBN * 128 bytes apart, 8-key groups 1024 bytes apart
 #pragma unroll
     for (int kk = 0; kk < kBN / 16; ++kk)
-      wgmma_pv<T, D>(o, pa[kk], make_smem_desc(v_addr + kk * 16 * 128, 1, kBN * 128, 1024), 1u);
+      wgmma_rs<T, D, true>(o, pa[kk], make_smem_desc(v_addr + kk * 16 * 128, 1, kBN * 128, 1024), 1u);
   };
   // mask and online softmax of tile n's S: P into pa, O rescaled
   auto softmax = [&](int n) {

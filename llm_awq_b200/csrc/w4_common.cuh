@@ -1,6 +1,7 @@
 // Shared device helpers for the sm_90a kernels: packed-format index math, exact int4 -> fp16/bf16
 // dequantisation, and one copy of every PTX wrapper more than one kernel uses (shared-memory loads,
-// cp.async, mbarrier, bulk copy, PDL, cluster, wgmma accumulator fences).
+// cp.async, mbarrier, bulk copy, PDL, cluster, wgmma accumulator fences, mma.sync m16n8k16).  The wgmma
+// instructions themselves are in tma_wgmma.cuh.
 //
 // Packed format (closed form of the reference packer awq/quantize/qmodule.py:26-65):
 // qweight is int16 [N/4, K].  Each 4-row x 64-k tile is one contiguous 128-byte segment
@@ -270,21 +271,18 @@ __device__ __forceinline__ void st_async_f32(uint32_t cluster_addr, float v, uin
 // ---------------------------------------------------------------- warp-level tensor-core MAC
 // D[16 x 8] = A[16 x 16] * B[16 x 8] + C, fp32 accumulate.  Not `volatile`: a pure function of its register
 // operands, so the compiler may interleave independent groups.  Used by the HBM-bound streaming and ring
-// kernels: rows of A are output channels (dequantised in registers), columns of B are tokens.
+// kernels: rows of A are output channels (dequantised in registers), columns of B are tokens.  The asm template must
+// be a string literal, so the type TY ("f16" / "bf16") comes in as a macro argument.
+#define B200AWQ_MMA_16816(TY)                                                                     \
+  asm("mma.sync.aligned.m16n8k16.row.col.f32." TY "." TY ".f32 "                                 \
+      "{%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%10,%11,%12,%13};"                                 \
+      : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3])                                            \
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1), "f"(c[0]), "f"(c[1]), "f"(c[2]), "f"(c[3]))
 template <typename T>
 __device__ __forceinline__ void mma_16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
                                           uint32_t b0, uint32_t b1, const float (&c)[4]) {
-  if constexpr (!TypeTraits<T>::kIsBf16) {
-    asm(
-        "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%10,%11,%12,%13};"
-        : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3])
-        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1), "f"(c[0]), "f"(c[1]), "f"(c[2]), "f"(c[3]));
-  } else {
-    asm(
-        "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%10,%11,%12,%13};"
-        : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3])
-        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1), "f"(c[0]), "f"(c[1]), "f"(c[2]), "f"(c[3]));
-  }
+  if constexpr (!TypeTraits<T>::kIsBf16) B200AWQ_MMA_16816("f16");
+  else B200AWQ_MMA_16816("bf16");
 }
 
 }  // namespace b200awq

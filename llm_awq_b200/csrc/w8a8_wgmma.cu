@@ -1,4 +1,4 @@
-// Tensor-core W8A8 GEMM for sm_90a: TMA -> 128-byte-swizzled shared memory -> wgmma.mma_async.s32.s8.s8 with both
+// Tensor-core W8A8 GEMM for sm_90a: TMA -> 128-byte-swizzled shared memory -> s8 x s8 -> s32 wgmma_ss with both
 // operands taken from shared-memory descriptors -> exact int32 accumulators -> the reference's fp32 epilogue -> fp16.
 //
 // Replaces the reference's dense_kernel0 / dense_kernel0_fuse_bias (w8a8/w8a8_gemm_cuda.cu; Ampere cp.async +
@@ -38,25 +38,6 @@ constexpr int kStageBytes = kXBytes + kWBytes;
 constexpr int kOutRow = kTN * 2 + 16;         // staged fp16 row (+ pad against bank conflicts)
 static_assert(kTM * kOutRow <= kStages * kStageBytes, "epilogue staging must fit in the pipeline buffers");
 constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 64 /*barriers*/;
-
-// D[64 x 128] (+)= A[64 x 32] * B[32 x 128], int8 x int8 -> int32, both operands K-major in shared memory
-__device__ __forceinline__ void wgmma_s8_n128(int (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,"
-      "%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,"
-      "%58,%59,%60,%61,%62,%63}, %64, %65, p;\n}\n"
-      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]),
-        "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]),
-        "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]),
-        "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]),
-        "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]),
-        "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]),
-        "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]),
-        "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
-      : "l"(adesc), "l"(bdesc), "r"(accum));
-}
 
 __device__ __forceinline__ float ldg_h(const __half* p) { return __half2float(__ldg(p)); }
 
@@ -177,7 +158,7 @@ w8a8_wgmma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constan
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < kTK / 32; ++kk)  // +32 B along k per instruction
-      wgmma_s8_n128(acc, adesc + (uint64_t)(kk * 2), bdesc + (uint64_t)(kk * 2), (kb | kk) != 0 ? 1u : 0u);
+      wgmma_ss(acc, adesc + (uint64_t)(kk * 2), bdesc + (uint64_t)(kk * 2), (kb | kk) != 0 ? 1u : 0u);
     wgmma_commit();
     wgmma_wait<1>();  // the previous stage's wgmmas have completed: its buffers may be refilled
     acc_fence(acc);
