@@ -321,6 +321,25 @@ int b200awq_sample_next_token(const float* logits, long long logits_row_stride, 
                               float repetition_penalty, float top_p, int top_k, int greedy, const float* uniforms,
                               long long* tokens, void* stream);
 
+/* The LM head: the decoder's final RMSNorm and the vocabulary projection in one launch, fp32 logits for
+ * b200awq_sample_next_token (tinychat/models/llama.py:353-354, 395, 412-413: `norm(h[:, -1:, :])`, `lm_head(h)`,
+ * `.float()`; DESIGN §3.13).  For i < m, v < vocab:
+ *   logits[i * vocab + v] = (float) rn_T( sum_j x^[i, j] * weight[v * k + j] )
+ * where x^ = x, or with gamma non-NULL exactly what b200awq_rmsnorm(x, gamma, eps) writes (fp16 clamp included); the
+ * sum is accumulated in fp32 in an order that depends on k alone (not on vocab, v, m, the other rows or the device),
+ * rounded once to T (fp16 overflow gives +-inf) and widened exactly.
+ *   x         [m, k] of T, row i at x + i * x_row_stride elements; x_row_stride >= k (else B200AWQ_ERR_SHAPE) and a
+ *             multiple of 8 (else B200AWQ_ERR_ALIGN), so that h[:, -1, :] of a [B, S, k] hidden state is read in place
+ *   gamma     [k] of T or NULL (no norm); eps finite and >= 0 when gamma is given (else B200AWQ_ERR_SHAPE)
+ *   weight    [vocab, k] of T, contiguous (an untied lm_head or a tied embedding)
+ *   logits    [m, vocab] fp32, contiguous; must not overlap x, gamma or weight (else B200AWQ_ERR_ALIGN)
+ * 1 <= m <= 8 (else B200AWQ_ERR_BATCH); vocab >= 1, 8 <= k <= 8192, k % 8 == 0 (else B200AWQ_ERR_SHAPE); x, gamma,
+ * weight and logits 16-byte aligned (else B200AWQ_ERR_ALIGN).  One launch, no workspace, no atomics, deterministic,
+ * safe under graph capture; x and gamma are read after the launch's dependency wait (the previous launch may write
+ * them), weight is a model constant streamed from before it, so the launch right before must not write it. */
+int b200awq_lm_head(const void* x, long long x_row_stride, const void* gamma, float eps, const void* weight, float* logits,
+                    int m, int vocab, int k, int dtype, void* stream);
+
 /* ---- W8A8 (int8 weights, int8 per-token activations): the vision-tower ops of the reference's extension
  * (csrc/pybind.cpp:30-37), called by awq/quantize/w8a8_linear.py and tinychat's QuantSiglipEncoder /
  * QuantInternVisionEncoder.  Scales are fp16 everywhere (the reference reads them as at::Half).  fp32 activations,

@@ -18,7 +18,7 @@ EXT = os.path.join(HERE, "plugin", "awq_inference_engine" + sysconfig.get_config
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
 KERNEL_SRCS = ("api.cu", "w4a16_decode.cu", "w4a16_ring.cu", "w4a16_stream.cu", "w4a16_wgmma.cu", "rmsnorm.cu", "silu_mul.cu", "attention.cu", "rope_neox.cu",
-               "rope_kv_store.cu", "sampling.cu",
+               "rope_kv_store.cu", "sampling.cu", "lm_head.cu",
                "w8a8_wgmma.cu", "w8a8_rowops.cu", "prefill_attention.cu", "splitkv_attention.cu")
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",

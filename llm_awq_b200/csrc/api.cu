@@ -430,6 +430,28 @@ int b200awq_sample_next_token(const float* logits, long long logits_row_stride, 
                                                    pdl_enabled(), static_cast<cudaStream_t>(stream)));
 }
 
+int b200awq_lm_head(const void* x, long long x_row_stride, const void* gamma, float eps, const void* weight, float* logits,
+                    int m, int vocab, int k, int dtype, void* stream) {
+  if (int e = check_dtype(dtype)) return e;
+  if (m < 1 || m > b200awq::kLmHeadMaxM) return B200AWQ_ERR_BATCH;
+  if (vocab < 1 || k < 8 || k > 8192 || k % 8 || x_row_stride < k) return B200AWQ_ERR_SHAPE;
+  if (!aligned16(x) || !aligned16(weight) || !aligned16(logits) || (gamma && !aligned16(gamma)) || x_row_stride % 8)
+    return B200AWQ_ERR_ALIGN;
+  if (gamma && !(std::isfinite(eps) && eps >= 0.f)) return B200AWQ_ERR_SHAPE;
+  // the logits are written while the inputs are read: they must not share a byte with any of them
+  const uintptr_t o = reinterpret_cast<uintptr_t>(logits), o_end = o + (uintptr_t)m * (uintptr_t)vocab * 4u;
+  auto overlaps = [o, o_end](const void* p, uintptr_t bytes) {
+    const uintptr_t b = reinterpret_cast<uintptr_t>(p);
+    return p && b < o_end && o < b + bytes;
+  };
+  if (overlaps(x, ((uintptr_t)(m - 1) * (uintptr_t)x_row_stride + (uintptr_t)k) * 2u) ||
+      overlaps(weight, (uintptr_t)vocab * (uintptr_t)k * 2u) || overlaps(gamma, (uintptr_t)k * 2u))
+    return B200AWQ_ERR_ALIGN;
+  if (int e = check_device()) return e;
+  return counted(b200awq::launch_lm_head(x, x_row_stride, gamma, eps, weight, logits, m, vocab, k, dtype, pdl_enabled(),
+                                         static_cast<cudaStream_t>(stream)));
+}
+
 int b200awq_rope_with_pos(const void* x, const float* freqs, void* y, int s, int b, int h, int d, int d2,
                           const long long in_strides[4], const long long out_strides[4], int dtype, void* stream) {
   if (int e = check_dtype(dtype)) return e;

@@ -728,6 +728,39 @@ torch::Tensor sample_next_token(const torch::Tensor& logits, c10::optional<torch
   return tokens;
 }
 
+// tinychat's tail in one launch (include/b200awq.h, b200awq_lm_head): the fp32 logits [m, vocab] of hidden [m, k]
+// (any row stride that is a multiple of 8, so h[:, -1, :] is read in place) against weight [vocab, k], after the final
+// RMSNorm when gamma [k] is given.  hidden, weight and gamma share one dtype and device.
+torch::Tensor lm_head_forward_cuda(const torch::Tensor& hidden, const torch::Tensor& weight, c10::optional<torch::Tensor> gamma,
+                                   double eps) {
+  const char* fn = "lm_head_forward_cuda";
+  TORCH_CHECK(hidden.is_cuda() && weight.is_cuda() && weight.device() == hidden.device(), fn,
+              ": hidden and weight must be CUDA tensors on one device");
+  const int dt = dtype_code(hidden, fn);
+  TORCH_CHECK(weight.scalar_type() == hidden.scalar_type(), fn, ": weight must have hidden's dtype");
+  TORCH_CHECK(hidden.dim() == 2 && (hidden.stride(1) == 1 || hidden.size(1) <= 1), fn,
+              ": hidden must be [m, k] with a contiguous last dimension");
+  TORCH_CHECK(weight.dim() == 2 && weight.is_contiguous() && weight.size(1) == hidden.size(1), fn,
+              ": weight must be a contiguous [vocab, k] matching hidden");
+  const int64_t m = hidden.size(0), k = hidden.size(1), vocab = weight.size(0);
+  TORCH_CHECK(m <= 8, fn, ": at most 8 rows, got ", m);
+  TORCH_CHECK(vocab <= INT32_MAX && k <= INT32_MAX, fn, ": sizes out of range");
+  const void* g = nullptr;
+  if (gamma.has_value()) {
+    TORCH_CHECK(gamma->is_cuda() && gamma->device() == hidden.device(), fn, ": gamma must be on hidden's device");
+    TORCH_CHECK(gamma->scalar_type() == hidden.scalar_type(), fn, ": gamma must have hidden's dtype");
+    TORCH_CHECK(gamma->is_contiguous() && gamma->numel() == k, fn, ": gamma must be contiguous with ", k, " elements");
+    g = gamma->data_ptr();
+  }
+  const c10::cuda::CUDAGuard guard(hidden.device());
+  torch::Tensor logits = torch::empty({m, vocab}, hidden.options().dtype(torch::kFloat32));
+  if (m == 0) return logits;
+  const long long stride = m == 1 ? (long long)k : (long long)hidden.stride(0);  // a single row's stride is never used
+  raise(b200awq_lm_head(hidden.data_ptr(), stride, g, (float)eps, weight.data_ptr(), logits.data_ptr<float>(), (int)m,
+                        (int)vocab, (int)k, dt, current_stream()));
+  return logits;
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "H100 (sm_90a) drop-in for llm-awq's awq_inference_engine (W4A16 and W8A8 paths)";
   m.def("gemm_forward_cuda_new", &gemm_forward_cuda_new, "New quantized GEMM kernel.");
@@ -783,6 +816,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         "tinychat's temperature, repetition penalty, top-p, top-k and the choice of the next token, one launch",
         py::arg("logits"), py::arg("prev_ids"), py::arg("temperature"), py::arg("repetition_penalty"), py::arg("top_p"),
         py::arg("top_k"), py::arg("greedy"), py::arg("uniforms") = py::none());
+  m.def("lm_head_forward_cuda", &lm_head_forward_cuda,
+        "fp32 logits of the LM head, optionally after the final RMSNorm, one launch", py::arg("hidden"), py::arg("weight"),
+        py::arg("gamma") = py::none(), py::arg("eps") = 1e-6);
   m.def("set_pdl",[](bool on) { return b200awq_set_pdl(on ? 1 : 0) != 0; }, "programmatic dependent launch on/off");
   m.def("launch_count", []() { return b200awq_launch_count(); }, "kernels launched by libb200awq so far");
   m.def("version", []() { return std::string(b200awq_version()); });

@@ -171,6 +171,12 @@ int launch_sample_next_token(const float* logits, long long logits_stride, int b
                              long long prev_stride, int n_prev, float temperature, float penalty, float top_p, int top_k,
                              int greedy, const float* uniforms, long long* tokens, bool pdl, cudaStream_t stream);
 
+// the LM head's fp32 logits of 1 <= m <= kLmHeadMaxM rows, RMSNorm prologue when gamma is non-null; arguments as
+// b200awq_lm_head, validated (lm_head.cu)
+constexpr int kLmHeadMaxM = 8;
+int launch_lm_head(const void* x, long long x_row_stride, const void* gamma, float eps, const void* weight, float* logits,
+                   int m, int vocab, int k, int dtype, bool pdl, cudaStream_t stream);
+
 // forward attention over many queries, D in {64, 72, 128}; arguments as b200awq_prefill_attention (prefill_attention.cu)
 int launch_prefill_attention(const void* q, const void* k, const void* v, void* out, const int* cu_q, const int* cu_k, int batch,
                              int seqlen_q, int seqlen_k, int heads, int kv_heads, int head_dim, const long long* q_strides,

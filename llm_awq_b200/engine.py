@@ -65,6 +65,8 @@ def lib() -> ctypes.CDLL:
         L.b200awq_rope_kv_store.restype = ci
         L.b200awq_sample_next_token.argtypes = [vp, ll, ci, ci, vp, ll, ci, fl, fl, fl, ci, ci, vp, vp, vp]
         L.b200awq_sample_next_token.restype = ci
+        L.b200awq_lm_head.argtypes = [vp, ll, vp, fl, vp, vp, ci, ci, ci, ci, vp]
+        L.b200awq_lm_head.restype = ci
         L.b200awq_rope_with_pos.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, vp, vp, ci, vp]
         L.b200awq_rope_with_pos.restype = ci
         L.b200awq_rotary_embedding_neox.argtypes = [vp, vp, vp, vp, ci, ci, ci, ci, ci, ctypes.c_longlong, ctypes.c_longlong, ci, vp]
